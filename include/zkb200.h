@@ -237,6 +237,20 @@ int zk_groth16_verify_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_
 /* same with device pointers; asynchronous on the context's stream (zk_ctx_sync reports a pending ZK_ERR_NOT_CANONICAL) */
 int zk_groth16_verify_batch_device(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs, const uint64_t *d_inputs,
                                    size_t n_inputs, uint8_t *d_verdicts);
+/* ---- Jubjub public inputs (what modules/zk-system/src/lib.rs:56-165 builds before verify_proof) ----------------
+ * Point::read + as_prime_order + into_xy (core/jubjub/src/curve/edwards.rs:92-164, 319-352) for n 32-byte encodings.
+ * xy: n * 2 canonical Fr (x then y; 4 LE u64 each); status[i]: 0 ok, 1 NotInField (y >= r), 2 NotOnCurve (no square root),
+ * 3 not in the prime-order subgroup (as_prime_order == None).  A rejected point's x and y are zero. */
+int zk_jubjub_into_xy(zk_ctx *ctx, size_t n, const uint8_t *points, uint64_t *xy, uint8_t *status);
+/* verify_confidential_proof / verify_anonymous_proof (modules/zk-system/src/lib.rs:56-165) for n transactions:
+ * points = n * n_points * 32 bytes in PublicInputBuilder push order; public inputs = (x0, y0, x1, y1, ...).
+ * verdicts as zk_groth16_verify_batch, plus 4 = a public-input point was rejected (the reference builds the inputs
+ * before Proof::read, so 4 takes precedence over 2 / 3).  ZK_ERR_MALFORMED_VK when 2 * n_points + 1 != ic.len(). */
+int zk_groth16_verify_points_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *proofs, const uint8_t *points,
+                                   size_t n_points, uint8_t *verdicts);
+/* same with device pointers; asynchronous on the context's stream */
+int zk_groth16_verify_points_batch_device(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs,
+                                          const uint8_t *d_points, size_t n_points, uint8_t *d_verdicts);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

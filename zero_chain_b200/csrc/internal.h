@@ -70,6 +70,7 @@ struct zk_ctx {
     DevBuf g_a, g_b, g_c, g_h, g_scal, g_misc;
     // verifier workspace (pairing.cu)
     DevBuf v_pts, v_stat, v_coef, v_f, v_part, v_io;
+    DevBuf v_jj;                   // zk_groth16_verify_points_batch: decoded public inputs and per-point status (jubjub.cu)
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;
     std::vector<cudaEvent_t> prof_events;   // pairs (start, stop)
@@ -118,6 +119,11 @@ int zk_check_err_flag(zk_ctx *ctx);
 void zk_launch_miller_lanes(cudaStream_t st, size_t n, const void *a, const void *acc, const void *c, const void *coef_b, const void *gamma, int gamma_inf,
                             const void *delta, int delta_inf, const uint8_t *status, void *f);
 void zk_launch_verify_final_lanes(cudaStream_t st, size_t n, const void *f, const void *alpha_beta, const uint8_t *status, uint8_t *verdict);
+// Jubjub public-input decoding (jubjub.cu): xy[2 p], xy[2 p + 1] = canonical x, y of encoding p, status[p] 0..3; then verdict
+// ZK_VERDICT_INPUT_REJECTED for every transaction i with a nonzero status[i * n_points + j]
+constexpr uint8_t ZK_VERDICT_INPUT_REJECTED = 4;
+void zk_launch_jubjub_into_xy(cudaStream_t st, const uint8_t *d_enc, size_t n, uint64_t *d_xy, uint8_t *d_status);
+void zk_launch_mark_rejected_inputs(cudaStream_t st, size_t n, size_t n_points, const uint8_t *d_status, uint8_t *d_verdicts);
 int zk_fr_to_mont(zk_ctx *ctx, const void *d_in, size_t n, void *d_out);
 int zk_fr_witness_to_mont(zk_ctx *ctx, const void *d_inputs, size_t n_in, const void *d_aux, size_t n_aux, size_t batch, void *d_z);
 int zk_fr_r1cs_eval(zk_ctx *ctx, const uint32_t *d_row_ptr, const uint32_t *d_col, const void *d_coeff, const void *d_z, size_t n_c, size_t n_in,

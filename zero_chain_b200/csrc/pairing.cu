@@ -5,6 +5,7 @@
 // Schedule for a batch of n proofs against one prepared key — every stage is a grid over independent work items, so a
 // block's worth of transactions fills the machine even though one pairing is a long serial computation:
 //   k_proof_decode_g1/g2   3n points: flags, x < q, y by square root, sign, r*P = O            (Proof::read)
+//   k_jubjub_into_xy       n * n_points Jubjub encodings -> the public inputs (only for zk_groth16_verify_points_batch; jubjub.cu)
 //   k_ic_partial           n * n_inputs items: x_ij * ic_j as 32 mixed additions from a per-key table of
 //                          d * 2^(8w) * ic_j (d = 1..255), then k_ic_sum: ic_0 + sum_j          (the public-input MSM)
 //   k_g2_prepare           n items: the 68 line coefficients of B_i                              (G2Affine::prepare)
@@ -307,26 +308,28 @@ extern "C" int zk_pvk_prepare(zk_ctx *ctx, const uint8_t *vk, size_t len, zk_pvk
     return ZK_OK;
 }
 
-// proofs / inputs / verdicts are device pointers
-extern "C" int zk_groth16_verify_batch_device(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs, const uint64_t *d_inputs,
-                                              size_t n_inputs, uint8_t *d_verdicts) {
-    if (!ctx || !k || (n && (!d_proofs || !d_verdicts)) || (n && n_inputs && !d_inputs)) { zk_set_error("zk_groth16_verify_batch: NULL argument"); return ZK_ERR_INVALID; }
-    if (n_inputs + 1 != k->n_ic) {     // verifier.rs:38-40
-        zk_set_error("MalformedVerifyingKey: %zu public inputs for a key with ic.len() = %zu", n_inputs, k->n_ic);
-        return ZK_ERR_MALFORMED_VK;
-    }
-    if (!n) return ZK_OK;
-    ZK_TRY(zk_use_device(ctx));
-    if (k->device != ctx->device) { zk_set_error("prepared key lives on device %d, context on %d", k->device, ctx->device); return ZK_ERR_INVALID; }
+// The verifier schedule behind zk_groth16_verify_batch_device and zk_groth16_verify_points_batch_device; all pointers are device
+// pointers.  Without d_points the public inputs are d_inputs (n * n_inputs canonical Fr).  With d_points (n * n_points Jubjub
+// encodings, n_inputs = 2 n_points) they are decoded first on the public-input strand into the context's workspace, and
+// transactions with a rejected point get verdict 4 after the final exponentiation.
+static int verify_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs, const uint64_t *d_inputs, size_t n_inputs,
+                        const uint8_t *d_points, size_t n_points, uint8_t *d_verdicts) {
     const size_t chunk = VERIFY_CHUNK;
     if (n > chunk) {                   // bound the workspace (19.6 KB of B coefficients per proof): slices run back to back on the stream
         for (size_t o = 0; o < n; o += chunk) {
             size_t m = n - o < chunk ? n - o : chunk;
-            ZK_TRY(zk_groth16_verify_batch_device(ctx, k, m, d_proofs + 192 * o, d_inputs + 4 * n_inputs * o, n_inputs, d_verdicts + o));
+            ZK_TRY(verify_batch(ctx, k, m, d_proofs + 192 * o, d_points ? nullptr : d_inputs + 4 * n_inputs * o, n_inputs,
+                                d_points ? d_points + 32 * n_points * o : nullptr, n_points, d_verdicts + o));
         }
         return ZK_OK;
     }
     cudaStream_t st = ctx->stream;
+    uint8_t *pt_stat = nullptr;
+    if (d_points) {                    // decoded inputs (64 B per point, 16-byte aligned), then one status byte per point
+        ZK_TRY(ctx->v_jj.reserve(n * n_points * 65));
+        d_inputs = ctx->v_jj.as<uint64_t>();
+        pt_stat = ctx->v_jj.as<uint8_t>() + n * n_points * 64;
+    }
     ZK_TRY(ctx->v_pts.reserve(n * (3 * sizeof(G1A) + sizeof(G2A))));
     ZK_TRY(ctx->v_stat.reserve(3 * n));
     ZK_TRY(ctx->v_coef.reserve(n * COEF_BYTES));
@@ -352,6 +355,7 @@ extern "C" int zk_groth16_verify_batch_device(zk_ctx *ctx, const zk_pvk *k, size
     ZK_CUDA(cudaStreamWaitEvent(s2, ev.e[0], 0)); ZK_CUDA(cudaStreamWaitEvent(s3, ev.e[0], 0));
     k_proof_decode_g1<<<grid(2 * n), PT, 0, s2>>>(d_proofs, n, a, c, stt);
     ZK_CUDA(cudaEventRecord(ev.e[1], s2));
+    if (d_points) zk_launch_jubjub_into_xy(s3, d_points, n * n_points, const_cast<uint64_t *>(d_inputs), pt_stat);
     if (n_inputs) k_ic_partial<<<grid(n * n_inputs), PT, 0, s3>>>(k->table, (const uint32_t *)d_inputs, n, n_inputs, part, ctx->d_err);
     k_ic_sum<<<grid(n), PT, 0, s3>>>(part, k->ic, n, n_inputs, acc);
     ZK_CUDA(cudaEventRecord(ev.e[2], s3));
@@ -365,8 +369,61 @@ extern "C" int zk_groth16_verify_batch_device(zk_ctx *ctx, const zk_pvk *k, size
         k_miller<<<grid(3 * n), PT, 0, st>>>(n, a, acc, c, coef, k->gamma, k->gamma_inf, k->delta, k->delta_inf, stt, f);
         k_verify_final<<<grid(n), PT, 0, st>>>(n, f, k->alpha_beta, stt, d_verdicts);
     }
+    if (d_points) zk_launch_mark_rejected_inputs(st, n, n_points, pt_stat, d_verdicts);
     ZK_CUDA(cudaGetLastError());
     return ZK_OK;
+}
+
+static int verify_on_key_device(zk_ctx *ctx, const zk_pvk *k) {
+    ZK_TRY(zk_use_device(ctx));
+    if (k->device != ctx->device) { zk_set_error("prepared key lives on device %d, context on %d", k->device, ctx->device); return ZK_ERR_INVALID; }
+    return ZK_OK;
+}
+
+// proofs / inputs / verdicts are device pointers
+extern "C" int zk_groth16_verify_batch_device(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs, const uint64_t *d_inputs,
+                                              size_t n_inputs, uint8_t *d_verdicts) {
+    if (!ctx || !k || (n && (!d_proofs || !d_verdicts)) || (n && n_inputs && !d_inputs)) { zk_set_error("zk_groth16_verify_batch: NULL argument"); return ZK_ERR_INVALID; }
+    if (n_inputs + 1 != k->n_ic) {     // verifier.rs:38-40
+        zk_set_error("MalformedVerifyingKey: %zu public inputs for a key with ic.len() = %zu", n_inputs, k->n_ic);
+        return ZK_ERR_MALFORMED_VK;
+    }
+    if (!n) return ZK_OK;
+    ZK_TRY(verify_on_key_device(ctx, k));
+    return verify_batch(ctx, k, n, d_proofs, d_inputs, n_inputs, nullptr, 0, d_verdicts);
+}
+
+// proofs / points / verdicts are device pointers
+extern "C" int zk_groth16_verify_points_batch_device(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs, const uint8_t *d_points,
+                                                     size_t n_points, uint8_t *d_verdicts) {
+    if (!ctx || !k || (n && (!d_proofs || !d_verdicts)) || (n && n_points && !d_points)) { zk_set_error("zk_groth16_verify_points_batch: NULL argument"); return ZK_ERR_INVALID; }
+    if (2 * n_points + 1 != k->n_ic) {
+        zk_set_error("MalformedVerifyingKey: %zu public-input points (%zu inputs) for a key with ic.len() = %zu", n_points, 2 * n_points, k->n_ic);
+        return ZK_ERR_MALFORMED_VK;
+    }
+    if (!n) return ZK_OK;
+    ZK_TRY(verify_on_key_device(ctx, k));
+    return verify_batch(ctx, k, n, d_proofs, nullptr, 2 * n_points, n_points ? d_points : nullptr, n_points, d_verdicts);
+}
+
+extern "C" int zk_groth16_verify_points_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *proofs, const uint8_t *points, size_t n_points,
+                                              uint8_t *verdicts) {
+    if (!ctx || !k || (n && (!proofs || !verdicts)) || (n && n_points && !points)) { zk_set_error("zk_groth16_verify_points_batch: NULL argument"); return ZK_ERR_INVALID; }
+    if (2 * n_points + 1 != k->n_ic) {
+        zk_set_error("MalformedVerifyingKey: %zu public-input points (%zu inputs) for a key with ic.len() = %zu", n_points, 2 * n_points, k->n_ic);
+        return ZK_ERR_MALFORMED_VK;
+    }
+    if (!n) return ZK_OK;
+    ZK_TRY(zk_use_device(ctx));
+    const size_t pt_bytes = n * n_points * 32;
+    ZK_TRY(ctx->v_io.reserve(n * 192 + pt_bytes + n + 64));
+    uint8_t *d = ctx->v_io.as<uint8_t>();
+    uint8_t *d_pts = d + ((n * 192 + 15) & ~(size_t)15), *d_out = d_pts + pt_bytes;
+    ZK_CUDA(cudaMemcpyAsync(d, proofs, n * 192, cudaMemcpyHostToDevice, ctx->stream));
+    if (pt_bytes) ZK_CUDA(cudaMemcpyAsync(d_pts, points, pt_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    ZK_TRY(zk_groth16_verify_points_batch_device(ctx, k, n, d, d_pts, n_points, d_out));
+    ZK_CUDA(cudaMemcpyAsync(verdicts, d_out, n, cudaMemcpyDeviceToHost, ctx->stream));
+    return zk_check_err_flag(ctx);      // synchronises
 }
 
 extern "C" int zk_groth16_verify_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *proofs, const uint64_t *inputs, size_t n_inputs,

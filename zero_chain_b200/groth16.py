@@ -337,6 +337,76 @@ def verify_proofs_device(pvk: PreparedVerifyingKey, n: int, d_proofs_ptr: int, d
                                                   C.c_void_p(d_verdicts_ptr)))
 
 
+# ---- Jubjub public inputs (modules/zk-system/src/lib.rs:56-165) ---------------------------------------------------------
+# zk_jubjub_into_xy status codes: Point::read -> NotInField / NotOnCurve, as_prime_order -> None
+JUBJUB_OK, JUBJUB_NOT_IN_FIELD, JUBJUB_NOT_ON_CURVE, JUBJUB_NOT_PRIME_ORDER = 0, 1, 2, 3
+VERDICT_INPUT_REJECTED = 4          # a public-input point was rejected (checked before Proof::read, so it wins over 2 / 3)
+ANONIMITY_SIZE = 12                 # core/proofs/src/constants.rs:1
+CONFIDENTIAL_POINTS, ANONYMOUS_POINTS = 11, 4 * ANONIMITY_SIZE + 4
+
+
+def jubjub_into_xy(ctx: Context, encodings: bytes):
+    """Point::read + as_prime_order + into_xy (core/jubjub/src/curve/edwards.rs:92-164, 319-352) for len/32 encodings.
+    Returns (xy uint64 (n, 2, 4): canonical x then y, zero when rejected; status uint8 (n,): JUBJUB_*)."""
+    n = len(encodings) // 32
+    assert len(encodings) == 32 * n
+    xy = np.zeros((max(n, 1), 2, 4), np.uint64)
+    st = np.zeros(max(n, 1), np.uint8)
+    enc = np.frombuffer(encodings, np.uint8) if n else np.zeros(1, np.uint8)
+    _ck(_lib.lib().zk_jubjub_into_xy(ctx._h, n, _p(enc), _p(xy), _p(st)))
+    return xy[:n], st[:n]
+
+
+def verify_proofs_with_points(pvk: PreparedVerifyingKey, proofs: bytes, points: bytes, n_points: int) -> list:
+    """verify_confidential_proof / verify_anonymous_proof (lib.rs:56-165) for len(proofs)/192 transactions: each one's public
+    inputs are the (x, y) of its n_points 32-byte Jubjub encodings, in PublicInputBuilder push order (confidential_points /
+    anonymous_points).  Verdicts as verify_proofs, plus VERDICT_INPUT_REJECTED; raises SynthesisError(MalformedVerifyingKey)
+    when 2 * n_points + 1 != ic.len()."""
+    n = len(proofs) // 192
+    assert len(proofs) == 192 * n and len(points) == 32 * n_points * n
+    pb = np.frombuffer(proofs, np.uint8) if n else np.zeros(1, np.uint8)
+    pt = np.frombuffer(points, np.uint8) if n * n_points else np.zeros(1, np.uint8)
+    out = np.zeros(max(n, 1), np.uint8)
+    _ck(_lib.lib().zk_groth16_verify_points_batch(pvk.ctx._h, pvk._h, n, _p(pb), _p(pt), n_points, _p(out)))
+    return [int(v) for v in out[:n]]
+
+
+def verify_proofs_with_points_device(pvk: PreparedVerifyingKey, n: int, d_proofs_ptr: int, d_points_ptr: int, n_points: int,
+                                     d_verdicts_ptr: int):
+    """The same on device pointers, asynchronous on the context's stream."""
+    _ck(_lib.lib().zk_groth16_verify_points_batch_device(pvk.ctx._h, pvk._h, n, C.c_void_p(d_proofs_ptr), C.c_void_p(d_points_ptr),
+                                                         n_points, C.c_void_p(d_verdicts_ptr)))
+
+
+def _pt32(b) -> bytes:
+    b = bytes(b)
+    assert len(b) == 32, len(b)
+    return b
+
+
+def _ct64(b) -> bytes:
+    b = bytes(b)
+    assert len(b) == 64, len(b)       # Ciphertext: left point then right point
+    return b
+
+
+def confidential_points(address_sender, address_recipient, amount_sender, amount_recipient, randomness, fee_sender,
+                        balance_sender, rvk, g_epoch, nonce) -> bytes:
+    """The 11 points verify_confidential_proof pushes (lib.rs:69-100), in its order: randomness goes before fee_sender, and
+    the 64-byte balance_sender ciphertext contributes its left, then its right point.  352 bytes."""
+    return b"".join([_pt32(address_sender), _pt32(address_recipient), _pt32(amount_sender), _pt32(amount_recipient),
+                     _pt32(randomness), _pt32(fee_sender), _ct64(balance_sender), _pt32(rvk), _pt32(g_epoch), _pt32(nonce)])
+
+
+def anonymous_points(enc_keys, left_ciphertexts, enc_balances, right_ciphertext, rvk, g_epoch, nonce) -> bytes:
+    """The 52 points verify_anonymous_proof pushes (lib.rs:128-153): 12 encryption keys, 12 left ciphertexts, the left points
+    of the 12 balance ciphertexts, then their right points, then right_ciphertext, rvk, g_epoch, nonce.  1664 bytes."""
+    assert len(enc_keys) == len(left_ciphertexts) == len(enc_balances) == ANONIMITY_SIZE
+    bal = [_ct64(c) for c in enc_balances]
+    return b"".join([_pt32(k) for k in enc_keys] + [_pt32(c) for c in left_ciphertexts] + [c[:32] for c in bal] +
+                    [c[32:] for c in bal] + [_pt32(right_ciphertext), _pt32(rvk), _pt32(g_epoch), _pt32(nonce)])
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96

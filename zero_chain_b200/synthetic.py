@@ -138,13 +138,17 @@ def densities(r: R1CS):
     return a_aux, b_in, b_aux
 
 
-def make_witness(r: R1CS, seed=1):
-    """Full assignment z = (inputs | aux) satisfying r; returns python ints."""
+def make_witness(r: R1CS, seed=1, inputs=None):
+    """Full assignment z = (inputs | aux) satisfying r; returns python ints.  inputs: the n_inputs - 1 public inputs after
+    ONE (random when None)."""
     rng = SplitMix64(seed ^ 0xabcdef)
     z = [0] * (r.n_inputs + r.n_aux)
     z[0] = 1
     for i in range(1, r.n_inputs):
         z[i] = rng.fr()
+    if inputs is not None:
+        assert len(inputs) == r.n_inputs - 1
+        z[1:r.n_inputs] = [int(v) % R for v in inputs]
     for x in range(r.n_bool):
         z[r.n_inputs + x] = rng.next() & 1
     dot = lambda row: sum(c * z[v] for v, c in row) % R
