@@ -109,9 +109,12 @@ static __global__ void k_col_scan(const uint32_t *__restrict__ tile_hist, uint32
     }
     sizes[g] = run;
 }
+// KEYED (coarse level of the two-level sort): each entry is stored as {payload, bucket key}, so that k_fine_sort reads the
+// key with the entry instead of gathering it from the digits array (a random 4-byte read costs a 32-byte sector)
+template <bool KEYED>
 static __global__ void __launch_bounds__(SORT_THREADS) k_scatter(const uint32_t *__restrict__ digits, uint64_t e_ws, int nbins, int shift,
                                                           const uint32_t *__restrict__ tile_off, const uint32_t *__restrict__ bucket_off,
-                                                          uint32_t *__restrict__ sorted, int tiles_per_ws) {
+                                                          void *__restrict__ sorted, int tiles_per_ws) {
     extern __shared__ uint32_t sh[];
     int tile = blockIdx.x, ws = blockIdx.y;
     const uint32_t *to = tile_off + ((size_t)ws * tiles_per_ws + tile) * nbins;
@@ -124,7 +127,9 @@ static __global__ void __launch_bounds__(SORT_THREADS) k_scatter(const uint32_t 
         uint32_t code = d[p];
         if (code != DIGIT_ZERO) {
             uint32_t pos = atomicAdd(&sh[(code & 0x7fffffffu) >> shift], 1u);
-            sorted[pos] = (uint32_t)p | (code & 0x80000000u);
+            const uint32_t entry = (uint32_t)p | (code & 0x80000000u);
+            if (KEYED) reinterpret_cast<uint2 *>(sorted)[pos] = make_uint2(entry, code & 0x7fffffffu);
+            else reinterpret_cast<uint32_t *>(sorted)[pos] = entry;
         }
     }
 }
@@ -132,22 +137,18 @@ static __global__ void __launch_bounds__(SORT_THREADS) k_scatter(const uint32_t 
 // Fine level of the two-level sort (windows above 16 bits: 2^(c-1) buckets no longer fit a shared-memory histogram).
 // One block per (coarse bin, domain): the entries of the coarse bin (already contiguous) are counted by the low `low`
 // bits of their key in shared memory, the counts are scanned, and the entries are scattered to their final places.
-// Writes bucket sizes and bucket offsets directly (no global scan needed); the digit of an entry is re-read from the
-// digits array through its position.
-static __global__ void __launch_bounds__(1024) k_fine_sort(const uint32_t *__restrict__ coarse_sorted, const uint32_t *__restrict__ coarse_off,
-                                                          const uint32_t *__restrict__ digits, uint64_t e_ws, int n_coarse, int low,
+// Writes bucket sizes and bucket offsets directly (no global scan needed); the bucket key of an entry comes with it from
+// k_scatter<true>, so both passes read the coarse bin contiguously.
+static __global__ void __launch_bounds__(1024) k_fine_sort(const uint2 *__restrict__ coarse_sorted, const uint32_t *__restrict__ coarse_off,
+                                                          int n_coarse, int low,
                                                           uint32_t *__restrict__ sizes, uint32_t *__restrict__ bucket_off, uint32_t *__restrict__ sorted) {
     __shared__ uint32_t hist[1024];
     __shared__ uint32_t wsum[32];
     const int cb = blockIdx.x, dom = blockIdx.y, g = dom * n_coarse + cb;
     const uint32_t r0 = coarse_off[g], r1 = coarse_off[g + 1], fmask = (1u << low) - 1u;
-    const uint32_t *d = digits + (size_t)dom * e_ws;
     hist[threadIdx.x] = 0;
     __syncthreads();
-    for (uint32_t i = r0 + threadIdx.x; i < r1; i += blockDim.x) {
-        uint32_t code = coarse_sorted[i];
-        atomicAdd(&hist[d[code & 0x7fffffffu] & fmask], 1u);
-    }
+    for (uint32_t i = r0 + threadIdx.x; i < r1; i += blockDim.x) atomicAdd(&hist[coarse_sorted[i].y & fmask], 1u);
     __syncthreads();
     // exclusive scan of the (<= 1024) counters: one per thread
     uint32_t v = threadIdx.x < (1u << low) ? hist[threadIdx.x] : 0, inc = v;
@@ -173,9 +174,8 @@ static __global__ void __launch_bounds__(1024) k_fine_sort(const uint32_t *__res
     if (cb == n_coarse - 1 && dom == (int)gridDim.y - 1 && threadIdx.x == 0) bucket_off[((size_t)g + 1) << low] = r1;
     __syncthreads();
     for (uint32_t i = r0 + threadIdx.x; i < r1; i += blockDim.x) {
-        uint32_t code = coarse_sorted[i];
-        uint32_t pos = atomicAdd(&hist[d[code & 0x7fffffffu] & fmask], 1u);
-        sorted[pos] = code;
+        const uint2 e = coarse_sorted[i];
+        sorted[atomicAdd(&hist[e.y & fmask], 1u)] = e.x;
     }
 }
 

@@ -64,7 +64,7 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
     size_t smem = (size_t)sort_bins * 4;
     if (smem > 48 * 1024) {
         ZK_CUDA(cudaFuncSetAttribute(k_tile_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ZK_CUDA(cudaFuncSetAttribute(k_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ZK_CUDA(cudaFuncSetAttribute(k_scatter<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 gs((unsigned)tiles, (unsigned)n_dom);
     if (!two_level) {
@@ -72,18 +72,18 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
         k_col_scan<<<(unsigned)((NB + 255) / 256), 256, 0, st>>>(ctx->tile_hist.as<uint32_t>(), ctx->tile_off.as<uint32_t>(), ctx->sizes.as<uint32_t>(),
                                                                 nbins, tiles, (int)n_dom);
         exclusive_scan<false>(ctx->sizes.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(), NB, ctx->scan_scratch.as<uint32_t>(), st);
-        k_scatter<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, nbins, 0, ctx->tile_off.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(),
+        k_scatter<false><<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, nbins, 0, ctx->tile_off.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(),
                                                   ctx->sorted.as<uint32_t>(), tiles);
     } else {
-        ZK_TRY(ctx->sorted2.reserve(E * 4));
+        ZK_TRY(ctx->sorted2.reserve(E * sizeof(uint2)));           // {entry, bucket key} per entry (k_scatter<true>)
         ZK_TRY(ctx->coarse_off.reserve((SB + 1) * 4)); ZK_TRY(ctx->coarse_sizes.reserve((SB + 1) * 4));
         k_tile_hist<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, sort_bins, low, ctx->tile_hist.as<uint32_t>(), tiles);
         k_col_scan<<<(unsigned)((SB + 255) / 256), 256, 0, st>>>(ctx->tile_hist.as<uint32_t>(), ctx->tile_off.as<uint32_t>(), ctx->coarse_sizes.as<uint32_t>(),
                                                                 sort_bins, tiles, (int)n_dom);
         exclusive_scan<false>(ctx->coarse_sizes.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(), SB, ctx->scan_scratch.as<uint32_t>(), st);
-        k_scatter<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, sort_bins, low, ctx->tile_off.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(),
-                                                  ctx->sorted2.as<uint32_t>(), tiles);
-        k_fine_sort<<<dim3(512, (unsigned)n_dom), 1024, 0, st>>>(ctx->sorted2.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(), digits, e_dom, 512, low,
+        k_scatter<true><<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, sort_bins, low, ctx->tile_off.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(),
+                                                        ctx->sorted2.p, tiles);
+        k_fine_sort<<<dim3(512, (unsigned)n_dom), 1024, 0, st>>>(ctx->sorted2.as<uint2>(), ctx->coarse_off.as<uint32_t>(), 512, low,
                                                                  ctx->sizes.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(), ctx->sorted.as<uint32_t>());
     }
     // 2b. batched-affine rounds (msm_batchaff.cuh): each round halves every bucket at ~6.4 products per addition instead of the 10
