@@ -251,6 +251,19 @@ int zk_groth16_verify_points_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, const
 /* same with device pointers; asynchronous on the context's stream */
 int zk_groth16_verify_points_batch_device(zk_ctx *ctx, const zk_pvk *k, size_t n, const uint8_t *d_proofs,
                                           const uint8_t *d_points, size_t n_points, uint8_t *d_verdicts);
+/* ---- RedJubjub transaction signatures (what impl Verify for RedjubjubSignature runs per extrinsic) ---------------
+ * PublicKey::try_from(vk) + PublicKey::verify(msg, sig, FixedGenerators::Diversifier) (core/primitives/src/signature.rs:65-82,
+ * core/jubjub/src/redjubjub.rs:127-155) for n signatures.
+ * vks: n * 32 B; sigs: n * 64 B (rbar | sbar); msgs: concatenated message bytes, message i = msgs[msg_off[i] .. msg_off[i+1]),
+ * so msg_off has n + 1 entries and msgs holds msg_off[n] bytes; messages may be empty and start at any byte.
+ * verdicts[i]: 1 = true; 0 = the equation fails; 2 = vk is not a curve point; 3 = rbar is not a curve point; 4 = sbar >= r_J.
+ * (Every value other than 1 is the reference's `false`.  When several apply, the lowest of 2 / 3 / 4 wins, in the
+ * reference's order.)  ZK_ERR_INVALID for a NULL pointer, or for offsets that decrease. */
+int zk_redjubjub_verify_batch(zk_ctx *ctx, size_t n, const uint8_t *vks, const uint8_t *sigs, const uint8_t *msgs,
+                              const uint64_t *msg_off, uint8_t *verdicts);
+/* the same with device pointers; asynchronous on the context's stream.  The offsets are not checked: they must not decrease. */
+int zk_redjubjub_verify_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_vks, const uint8_t *d_sigs, const uint8_t *d_msgs,
+                                     const uint64_t *d_msg_off, uint8_t *d_verdicts);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

@@ -70,6 +70,8 @@ SIGNATURES = {
     "zk_jubjub_into_xy": (i32, [vp, sz, vp, vp, vp]),
     "zk_groth16_verify_points_batch": (i32, [vp, vp, sz, vp, vp, sz, vp]),
     "zk_groth16_verify_points_batch_device": (i32, [vp, vp, sz, vp, vp, sz, vp]),
+    "zk_redjubjub_verify_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_redjubjub_verify_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),
 }
 

@@ -114,10 +114,9 @@ ZK_DEV Ext ext_mul_order(const Ext &p, const Fr &d2) {
     return acc;
 }
 
-// Point::read + as_prime_order + into_xy of one 32-byte encoding given as 8 little-endian words.  On JJ_OK, x / y are the
-// canonical (non-Montgomery) coordinates; otherwise they are zero.
-ZK_DEV int jubjub_into_xy(const uint32_t *enc, Fr &x_out, Fr &y_out) {
-    x_out = Fr::zero(); y_out = Fr::zero();
+// Point::read of one 32-byte encoding given as 8 little-endian words, with no subgroup test (the Unknown order).  On JJ_OK,
+// p = (x : y : 1 : xy) in Montgomery form; otherwise JJ_NOT_IN_FIELD or JJ_NOT_ON_CURVE and p is unset.
+ZK_DEV int jubjub_read(const uint32_t *enc, Ext &p) {
     Fr yc;
 #pragma unroll
     for (int i = 0; i < 8; i++) yc.l[i] = enc[i];
@@ -132,12 +131,20 @@ ZK_DEV int jubjub_into_xy(const uint32_t *enc, Fr &x_out, Fr &y_out) {
     Fr u = (y2 - one).dbl() * den.inverse();
     Fr x;
     if (!fr_sqrt(u, x)) return JJ_NOT_ON_CURVE;
-    Fr xc = x.to_canonical();
-    if ((xc.l[0] & 1u) != sign) { x = x.neg(); xc = xc.neg(); }   // 0 stays 0 (edwards.rs:143-145)
-    Ext p;
+    if ((x.to_canonical().l[0] & 1u) != sign) x = x.neg();   // 0 stays 0 (edwards.rs:143-145)
     p.x = x; p.y = y; p.z = one; p.t = x * y;
-    if (!ext_is_identity(ext_mul_order(p, d2))) return JJ_NOT_PRIME_ORDER;
-    x_out = xc; y_out = yc;
+    return JJ_OK;
+}
+
+// Point::read + as_prime_order + into_xy of one 32-byte encoding given as 8 little-endian words.  On JJ_OK, x / y are the
+// canonical (non-Montgomery) coordinates; otherwise they are zero.
+ZK_DEV int jubjub_into_xy(const uint32_t *enc, Fr &x_out, Fr &y_out) {
+    x_out = Fr::zero(); y_out = Fr::zero();
+    Ext p;
+    const int s = jubjub_read(enc, p);
+    if (s != JJ_OK) return s;
+    if (!ext_is_identity(ext_mul_order(p, jj_d2()))) return JJ_NOT_PRIME_ORDER;
+    x_out = p.x.to_canonical(); y_out = p.y.to_canonical();
     return JJ_OK;
 }
 

@@ -407,6 +407,46 @@ def anonymous_points(enc_keys, left_ciphertexts, enc_balances, right_ciphertext,
                     [c[32:] for c in bal] + [_pt32(right_ciphertext), _pt32(rvk), _pt32(g_epoch), _pt32(nonce)])
 
 
+# ---- RedJubjub transaction signatures (core/primitives/src/signature.rs:65-82) ------------------------------------------
+# zk_redjubjub_verify_batch verdicts; every value but REDJUBJUB_OK is the reference's `false`
+REDJUBJUB_BAD_EQUATION, REDJUBJUB_OK, REDJUBJUB_BAD_VK, REDJUBJUB_BAD_R, REDJUBJUB_BAD_S = 0, 1, 2, 3, 4
+
+
+def _cat(items, size: int) -> bytes:
+    b = bytes(items) if isinstance(items, (bytes, bytearray, memoryview)) else b"".join(bytes(x) for x in items)
+    assert len(b) % size == 0, len(b)
+    return b
+
+
+def message_offsets(msgs) -> np.ndarray:
+    """The n + 1 offsets of the concatenated messages (uint64)."""
+    off = np.zeros(len(msgs) + 1, np.uint64)
+    np.cumsum([len(m) for m in msgs], out=off[1:])
+    return off
+
+
+def redjubjub_verify(ctx: Context, vks, sigs, msgs) -> list:
+    """PublicKey::verify(msg, sig, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:127-155) for each signature.
+    vks: 32-byte keys, sigs: 64-byte signatures (rbar | sbar), each a list or one concatenation; msgs: a list of byte strings.
+    Returns the REDJUBJUB_* verdict of each."""
+    vk, sg = _cat(vks, 32), _cat(sigs, 64)
+    n = len(msgs)
+    assert len(vk) == 32 * n and len(sg) == 64 * n
+    mb = b"".join(bytes(m) for m in msgs)
+    out = np.zeros(max(n, 1), np.uint8)
+    off = message_offsets(msgs)
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    _ck(_lib.lib().zk_redjubjub_verify_batch(ctx._h, n, _p(buf(vk)), _p(buf(sg)), _p(buf(mb)), _p(off), _p(out)))
+    return [int(v) for v in out[:n]]
+
+
+def redjubjub_verify_device(ctx: Context, n: int, d_vks_ptr: int, d_sigs_ptr: int, d_msgs_ptr: int, d_msg_off_ptr: int,
+                            d_verdicts_ptr: int):
+    """The same on device pointers (d_msg_off: n + 1 uint64 offsets), asynchronous on the context's stream."""
+    _ck(_lib.lib().zk_redjubjub_verify_batch_device(ctx._h, n, C.c_void_p(d_vks_ptr), C.c_void_p(d_sigs_ptr), C.c_void_p(d_msgs_ptr),
+                                                    C.c_void_p(d_msg_off_ptr), C.c_void_p(d_verdicts_ptr)))
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96
