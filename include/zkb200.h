@@ -264,6 +264,23 @@ int zk_redjubjub_verify_batch(zk_ctx *ctx, size_t n, const uint8_t *vks, const u
 /* the same with device pointers; asynchronous on the context's stream.  The offsets are not checked: they must not decrease. */
 int zk_redjubjub_verify_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_vks, const uint8_t *d_sigs, const uint8_t *d_msgs,
                                      const uint64_t *d_msg_off, uint8_t *d_verdicts);
+/* ---- lifted-ElGamal balance decryption (what zface's BalanceQuery runs before every transfer) --------------------
+ * DecryptionKey::read + Ciphertext::read (+ Ciphertext::read of the pending transfer and Ciphertext::add) +
+ * Ciphertext::decrypt(dk, FixedGenerators::Diversifier)  (core/keys/src/lib.rs:125-132, core/crypto/src/elgamal.rs:87-136,
+ * zface/src/utils/getter.rs:135-175) for n ciphertexts.
+ * dks: n * 32 B (Fs, little-endian); cts: n * 64 B (left | right); pending: NULL (none) or n * 64 B, added to cts first.
+ * values[i]: the amount when status[i] == 0, else 0.
+ * status[i]: 0 = Some(values[i]); 1 = None (no i < 1 000 000 with i P_G = left - dk right); 2 = dk >= r_J;
+ *            3 = cts[i] fails Ciphertext::read (either point: y >= r, not on the curve, or not of prime order);
+ *            4 = pending[i] fails Ciphertext::read.  When several apply, the lowest of 2 / 3 / 4 wins, in zface's order.
+ * ZK_ERR_INVALID for a NULL ctx / dks / cts / values / status when n > 0.  The first call on a context builds the table of
+ * the 10^6 multiples of P_G on the device; it stays resident until zk_ctx_destroy: 32 MB of encodings and an 8 MB index
+ * (about 45 MB with the allocator's headroom), plus 96 MB of scratch while it is built. */
+int zk_elgamal_decrypt_batch(zk_ctx *ctx, size_t n, const uint8_t *dks, const uint8_t *cts, const uint8_t *pending,
+                             uint32_t *values, uint8_t *status);
+/* the same with device pointers (d_values 4-byte aligned); asynchronous on the context's stream */
+int zk_elgamal_decrypt_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_dks, const uint8_t *d_cts, const uint8_t *d_pending,
+                                    uint32_t *d_values, uint8_t *d_status);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

@@ -71,6 +71,9 @@ struct zk_ctx {
     // verifier workspace (pairing.cu)
     DevBuf v_pts, v_stat, v_coef, v_f, v_part, v_io;
     DevBuf v_jj;                   // zk_groth16_verify_points_batch: decoded public inputs and per-point status (jubjub.cu)
+    // zk_elgamal_decrypt_batch (elgamal.cu): the encodings of i P_G for i < 10^6 and their index, built by the first call
+    DevBuf eg_table, eg_index;
+    bool eg_ready = false;
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;
     std::vector<cudaEvent_t> prof_events;   // pairs (start, stop)

@@ -447,6 +447,39 @@ def redjubjub_verify_device(ctx: Context, n: int, d_vks_ptr: int, d_sigs_ptr: in
                                                     C.c_void_p(d_msg_off_ptr), C.c_void_p(d_verdicts_ptr)))
 
 
+# ---- lifted-ElGamal balance decryption (core/crypto/src/elgamal.rs:87-136, zface/src/utils/getter.rs:135-175) ------------
+# zk_elgamal_decrypt_batch statuses: Some(value), None, DecryptionKey::read fails, Ciphertext::read of the balance / of the
+# pending transfer fails
+ELGAMAL_OK, ELGAMAL_NOT_FOUND, ELGAMAL_BAD_KEY, ELGAMAL_BAD_BALANCE, ELGAMAL_BAD_PENDING = 0, 1, 2, 3, 4
+ELGAMAL_BOUND = 1_000_000                          # the reference's search range, elgamal.rs:102
+ELGAMAL_ZERO = (b"\x01" + bytes(31)) * 2           # Ciphertext::zero(): two identities, what zface uses for an empty slot
+
+
+def elgamal_decrypt(ctx: Context, dks, cts, pending=None):
+    """Ciphertext::decrypt(dk, FixedGenerators::Diversifier) of each ciphertext, after adding its pending transfer if
+    `pending` is given.  dks: 32-byte keys, cts / pending: 64-byte ciphertexts, each a list or one concatenation.
+    Returns (statuses, values): the ELGAMAL_* status of each, and its amount (0 unless the status is ELGAMAL_OK)."""
+    dk, ct = _cat(dks, 32), _cat(cts, 64)
+    n = len(dk) // 32
+    assert len(ct) == 64 * n
+    pd = None if pending is None else _cat(pending, 64)
+    assert pd is None or len(pd) == 64 * n
+    values = np.zeros(max(n, 1), np.uint32)
+    st = np.zeros(max(n, 1), np.uint8)
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    _ck(_lib.lib().zk_elgamal_decrypt_batch(ctx._h, n, _p(buf(dk)), _p(buf(ct)), None if pd is None else _p(buf(pd)), _p(values), _p(st)))
+    return [int(s) for s in st[:n]], [int(v) for v in values[:n]]
+
+
+def elgamal_decrypt_device(ctx: Context, n: int, d_dks_ptr: int, d_cts_ptr: int, d_pending_ptr: int, d_values_ptr: int,
+                           d_status_ptr: int):
+    """The same on device pointers (d_pending = 0: no pending transfers; d_values: n uint32), asynchronous on the context's
+    stream."""
+    _ck(_lib.lib().zk_elgamal_decrypt_batch_device(ctx._h, n, C.c_void_p(d_dks_ptr), C.c_void_p(d_cts_ptr),
+                                                   C.c_void_p(d_pending_ptr) if d_pending_ptr else None, C.c_void_p(d_values_ptr),
+                                                   C.c_void_p(d_status_ptr)))
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96
