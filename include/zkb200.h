@@ -264,6 +264,33 @@ int zk_redjubjub_verify_batch(zk_ctx *ctx, size_t n, const uint8_t *vks, const u
 /* the same with device pointers; asynchronous on the context's stream.  The offsets are not checked: they must not decrease. */
 int zk_redjubjub_verify_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_vks, const uint8_t *d_sigs, const uint8_t *d_msgs,
                                      const uint64_t *d_msg_off, uint8_t *d_verdicts);
+/* sum_i scalars[i] * P_i over Jubjub (edwards::Point<Unknown>::mul + add).  points: n * 32 B Point::write encodings,
+ * read without a subgroup test; scalars: n * 32 B little-endian canonical Fs (< r_J); out: 32 B Point::write.
+ * ZK_ERR_DECODE (zk_last_error names the first bad index) for a point that fails Point::read, ZK_ERR_NOT_CANONICAL for a
+ * scalar >= r_J (checked first), ZK_ERR_INVALID for NULL arguments with n > 0 or n > 2^26.  n = 0 gives the identity. */
+int zk_jubjub_msm(zk_ctx *ctx, size_t n, const uint8_t *points, const uint8_t *scalars, uint8_t out[32]);
+/* redjubjub::batch_verify(rng, batch, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:166-204) for n entries,
+ * with the per-entry randomizers z_i (the reference's E::Fs::rand(rng)) supplied by the caller: n * 32 B canonical Fs.
+ * vks / sigs / msgs / msg_off exactly as zk_redjubjub_verify_batch.  On return:
+ *   *verdict = 1  [8](sum z_i R_i + sum (z_i c_i) vk_i - (sum z_i S_i) P_G) == O      (the reference's true; also for n = 0)
+ *            = 0  the combined equation fails
+ *            = 2 / 3 / 4  some entry's vk / rbar / sbar is rejected (the codes of zk_redjubjub_verify_batch);
+ *              *first_bad (may be NULL) = the lowest such index, and the code is that entry's, in the per-signature order.
+ *   *first_bad = n when no entry is rejected.
+ * The z_i MUST be unpredictable to the signers (drawn from a cryptographic RNG after the batch is fixed): the check only
+ * bounds a forged entry's chance of passing by ~1 / r_J over the draw of z, and a z_i = 0 lets any entry i pass.  A verdict
+ * other than 1 does not say which entry is wrong beyond the first rejected encoding: callers that need per-signature
+ * verdicts fall back to zk_redjubjub_verify_batch.
+ * ZK_ERR_NOT_CANONICAL for a z_i >= r_J; ZK_ERR_INVALID as zk_redjubjub_verify_batch (NULL, decreasing offsets) or for
+ * n >= 2^25. */
+int zk_redjubjub_batch_verify(zk_ctx *ctx, size_t n, const uint8_t *vks, const uint8_t *sigs, const uint8_t *msgs,
+                              const uint64_t *msg_off, const uint8_t *zs, uint8_t *verdict, uint64_t *first_bad);
+/* device pointers; asynchronous on the context's stream; d_verdict / d_first_bad in device memory (d_first_bad 8-byte
+ * aligned, may be NULL).  The offsets and the z_i are not checked on the host: an entry with z_i >= r_J is rejected on the
+ * device with *d_verdict = 5, ahead of that entry's own checks. */
+int zk_redjubjub_batch_verify_device(zk_ctx *ctx, size_t n, const uint8_t *d_vks, const uint8_t *d_sigs,
+                                     const uint8_t *d_msgs, const uint64_t *d_msg_off, const uint8_t *d_zs,
+                                     uint8_t *d_verdict, uint64_t *d_first_bad);
 /* ---- lifted-ElGamal balance decryption (what zface's BalanceQuery runs before every transfer) --------------------
  * DecryptionKey::read + Ciphertext::read (+ Ciphertext::read of the pending transfer and Ciphertext::add) +
  * Ciphertext::decrypt(dk, FixedGenerators::Diversifier)  (core/keys/src/lib.rs:125-132, core/crypto/src/elgamal.rs:87-136,

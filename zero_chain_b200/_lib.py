@@ -72,6 +72,9 @@ SIGNATURES = {
     "zk_groth16_verify_points_batch_device": (i32, [vp, vp, sz, vp, vp, sz, vp]),
     "zk_redjubjub_verify_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_redjubjub_verify_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_jubjub_msm": (i32, [vp, sz, vp, vp, vp]),
+    "zk_redjubjub_batch_verify": (i32, [vp, sz, vp, vp, vp, vp, vp, vp, vp]),
+    "zk_redjubjub_batch_verify_device": (i32, [vp, sz, vp, vp, vp, vp, vp, vp, vp]),
     "zk_elgamal_decrypt_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_elgamal_decrypt_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),

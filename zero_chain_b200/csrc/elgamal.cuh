@@ -52,15 +52,6 @@ ZK_DEV Niels niels_pg() {
     return q;
 }
 
-// Point::write (edwards.rs:190-206) of the affine point (x, y) in Montgomery form: canonical y, the parity of x in bit 255
-ZK_DEV void jubjub_encode(const Fr &x, const Fr &y, uint32_t *enc) {
-    const Fr yc = y.to_canonical();
-    const uint32_t sign = x.to_canonical().l[0] & 1u;
-#pragma unroll
-    for (int i = 0; i < 8; i++) enc[i] = yc.l[i];
-    enc[7] |= sign << 31;
-}
-
 ZK_DEV void fr_store(uint32_t *dst, const Fr &a) {
 #pragma unroll
     for (int i = 0; i < 8; i++) dst[i] = a.l[i];

@@ -74,6 +74,7 @@ struct zk_ctx {
     // zk_elgamal_decrypt_batch (elgamal.cu): the encodings of i P_G for i < 10^6 and their index, built by the first call
     DevBuf eg_table, eg_index;
     bool eg_ready = false;
+    DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;
     std::vector<cudaEvent_t> prof_events;   // pairs (start, stop)

@@ -136,6 +136,15 @@ ZK_DEV int jubjub_read(const uint32_t *enc, Ext &p) {
     return JJ_OK;
 }
 
+// Point::write (edwards.rs:190-206) of the affine point (x, y) in Montgomery form: canonical y, the parity of x in bit 255
+ZK_DEV void jubjub_encode(const Fr &x, const Fr &y, uint32_t *enc) {
+    const Fr yc = y.to_canonical();
+    const uint32_t sign = x.to_canonical().l[0] & 1u;
+#pragma unroll
+    for (int i = 0; i < 8; i++) enc[i] = yc.l[i];
+    enc[7] |= sign << 31;
+}
+
 // Point::read + as_prime_order + into_xy of one 32-byte encoding given as 8 little-endian words.  On JJ_OK, x / y are the
 // canonical (non-Montgomery) coordinates; otherwise they are zero.
 ZK_DEV int jubjub_into_xy(const uint32_t *enc, Fr &x_out, Fr &y_out) {

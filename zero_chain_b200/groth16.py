@@ -447,6 +447,72 @@ def redjubjub_verify_device(ctx: Context, n: int, d_vks_ptr: int, d_sigs_ptr: in
                                                     C.c_void_p(d_msg_off_ptr), C.c_void_p(d_verdicts_ptr)))
 
 
+# zk_redjubjub_batch_verify_device only: some z_i >= r_J (the host form raises ZK_ERR_NOT_CANONICAL instead)
+REDJUBJUB_BAD_Z = 5
+
+
+def jubjub_msm(ctx: Context, points, scalars) -> bytes:
+    """sum_i scalars[i] P_i over Jubjub (edwards::Point<Unknown>): points are 32-byte Point::write encodings, read without a
+    subgroup test; scalars are 32-byte little-endian Fs values < r_J (or ints).  Returns the 32-byte encoding of the sum."""
+    pt = _cat(points, 32)
+    if not isinstance(scalars, (bytes, bytearray, memoryview)):
+        scalars = [s.to_bytes(32, "little") if isinstance(s, int) else s for s in scalars]
+    sc = _cat(scalars, 32)
+    n = len(pt) // 32
+    assert len(sc) == 32 * n
+    out = np.zeros(32, np.uint8)
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    _ck(_lib.lib().zk_jubjub_msm(ctx._h, n, _p(buf(pt)), _p(buf(sc)), _p(out)))
+    return out.tobytes()
+
+
+def random_batch_scalars(n: int) -> bytes:
+    """n uniform Fs values from the operating system's CSPRNG (E::Fs::rand), 32 bytes each: the z_i of a batch check."""
+    r_j = 0x0e7db4ea6533afa906673b0101343b00a6682093ccc81082d0970e5ed6f72cb7
+    return b"".join((int.from_bytes(secrets.token_bytes(64), "little") % r_j).to_bytes(32, "little") for _ in range(n))
+
+
+def redjubjub_batch_verify(ctx: Context, vks, sigs, msgs, zs=None):
+    """redjubjub::batch_verify(rng, batch, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:166-204) with the
+    randomizers zs (32-byte canonical Fs each, or one concatenation; None draws them with random_batch_scalars).
+    Returns (verdict, first_bad): verdict 1 when the batch passes, 0 when the combined equation fails, or the
+    REDJUBJUB_BAD_VK / _R / _S code of the lowest rejected entry, whose index is first_bad (None otherwise)."""
+    vk, sg = _cat(vks, 32), _cat(sigs, 64)
+    n = len(msgs)
+    assert len(vk) == 32 * n and len(sg) == 64 * n
+    z = random_batch_scalars(n) if zs is None else _cat(zs, 32)
+    assert len(z) == 32 * n
+    mb = b"".join(bytes(m) for m in msgs)
+    off = message_offsets(msgs)
+    verdict = np.zeros(1, np.uint8)
+    first = np.zeros(1, np.uint64)
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    _ck(_lib.lib().zk_redjubjub_batch_verify(ctx._h, n, _p(buf(vk)), _p(buf(sg)), _p(buf(mb)), _p(off), _p(buf(z)), _p(verdict), _p(first)))
+    v = int(verdict[0])
+    return v, (int(first[0]) if v not in (REDJUBJUB_OK, REDJUBJUB_BAD_EQUATION) else None)
+
+
+def redjubjub_batch_verify_device(ctx: Context, n: int, d_vks_ptr: int, d_sigs_ptr: int, d_msgs_ptr: int, d_msg_off_ptr: int,
+                                  d_zs_ptr: int, d_verdict_ptr: int, d_first_bad_ptr: int = 0):
+    """The same on device pointers (d_msg_off: n + 1 uint64 offsets; d_zs: n * 32 bytes; d_verdict: one byte; d_first_bad:
+    one uint64 or 0), asynchronous on the context's stream."""
+    _ck(_lib.lib().zk_redjubjub_batch_verify_device(ctx._h, n, C.c_void_p(d_vks_ptr), C.c_void_p(d_sigs_ptr), C.c_void_p(d_msgs_ptr),
+                                                    C.c_void_p(d_msg_off_ptr), C.c_void_p(d_zs_ptr), C.c_void_p(d_verdict_ptr),
+                                                    C.c_void_p(d_first_bad_ptr) if d_first_bad_ptr else None))
+
+
+def redjubjub_verify_batched(ctx: Context, vks, sigs, msgs, zs=None) -> list:
+    """Per-signature verdicts, as redjubjub_verify returns them, through one batch check first: when the batch passes every
+    verdict is REDJUBJUB_OK, otherwise redjubjub_verify decides each signature.  The one difference from redjubjub_verify
+    is the reference's own soundness error: a batch with a bad signature passes with probability ~1 / r_J over the draw of
+    zs, so zs must be unpredictable to the signers (None draws them with random_batch_scalars)."""
+    n = len(msgs)
+    verdict, _ = redjubjub_batch_verify(ctx, vks, sigs, msgs, zs)
+    if verdict == REDJUBJUB_OK:
+        return [REDJUBJUB_OK] * n
+    return redjubjub_verify(ctx, vks, sigs, msgs)
+
+
 # ---- lifted-ElGamal balance decryption (core/crypto/src/elgamal.rs:87-136, zface/src/utils/getter.rs:135-175) ------------
 # zk_elgamal_decrypt_batch statuses: Some(value), None, DecryptionKey::read fails, Ciphertext::read of the balance / of the
 # pending transfer fails
