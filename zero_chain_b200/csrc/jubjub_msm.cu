@@ -298,10 +298,10 @@ static int jm_msm_run(zk_ctx *ctx, const JmPlan &p) {
                                                                  reinterpret_cast<int *>(small));
     // counting sort, one domain per window: entries grouped by (window, bucket)
     const size_t shm = 4 * (size_t)p.nb;
-    zkmsm::k_tile_hist<<<dim3(p.tiles, p.W), zkmsm::SORT_THREADS, shm, st>>>(digits, p.n, (int)p.nb, 0, hist, (int)p.tiles);
+    zkmsm::k_tile_hist<<<dim3(p.tiles, p.W), zkmsm::SORT_THREADS, shm, st>>>(digits, p.n, (int)p.nb, 0, hist, (int)p.tiles, zkmsm::TILE, false);
     zkmsm::k_col_scan<<<grid(p.NB, 256), 256, 0, st>>>(hist, toff, sizes, (int)p.nb, (int)p.tiles, p.W);
     zkmsm::exclusive_scan<false>(sizes, boff, p.NB, scan, st);
-    zkmsm::k_scatter<false><<<dim3(p.tiles, p.W), zkmsm::SORT_THREADS, shm, st>>>(digits, p.n, (int)p.nb, 0, toff, boff, sorted, (int)p.tiles);
+    zkmsm::k_scatter<<<dim3(p.tiles, p.W), zkmsm::SORT_THREADS, shm, st>>>(digits, p.n, (int)p.nb, toff, boff, sorted, (int)p.tiles, zkmsm::TILE);
     // buckets: runs of <= JM_RUN entries, then each bucket's runs folded
     k_jm_task_counts<<<grid(p.NB, 256), 256, 0, st>>>(sizes, p.NB, tcount);
     zkmsm::exclusive_scan<false>(tcount, task, p.NB, scan, st);

@@ -8,6 +8,8 @@
 //   2. k_tile_hist      per-tile bucket histograms in SHARED MEMORY (2^(c-1) counters, no global atomics)
 //      k_col_scan       per-bucket prefix over tiles;  scan -> bucket offsets
 //      k_scatter        counting-sort scatter with shared-memory cursors -> entries grouped by bucket
+//      (windows above 16 bits: k_tile_hist bins by the high 9 key bits over many small tiles, k_bin_scan scans the
+//      tiles, k_coarse_scatter groups each chunk by bin before storing it, k_fine_sort finishes each bin by the low bits)
 //   3. k_accumulate     one thread per <= TASK_LEN entries of one bucket: gathers affine bases from HBM
 //                       (software-prefetched), mixed additions into an XYZZ accumulator in registers
 //      k_combine_*      fold the bucket's task partials (thread per bucket; warp per heavy bucket)
@@ -28,8 +30,11 @@
 
 namespace zkmsm {
 
-constexpr int TILE = 131072;       // entries per sort tile (one tile ~ one CTA of a single wave at 2^20 x 16 windows)
+constexpr int TILE = 131072;       // entries per tile of the one-level sort (one tile ~ one CTA of a single wave at 2^20 x 16 windows)
 constexpr int SORT_THREADS = 1024;
+// Coarse level of the two-level sort: 256-thread blocks, tiles sized so that the grid is at least two full waves of
+// them (coarse_tile_len)
+constexpr int COARSE_THREADS = 256;
 constexpr uint32_t DIGIT_ZERO = 0xffffffffu;
 
 // ---- 1. digits ---------------------------------------------------------------------------------
@@ -77,22 +82,60 @@ static __global__ void k_msm_digits(const uint32_t *__restrict__ scalars, uint32
 }
 
 // ---- 2. counting sort --------------------------------------------------------------------------
+// Block-wide walk over cnt consecutive elements of s (aligned to sizeof(T)): f(element, index) for every element, with
+// 16-byte loads (4 digit codes or 2 {entry, key} pairs), U of them issued per thread before any is used, so that each
+// thread keeps U x 16 bytes in flight.  The few elements before the first 16-byte boundary and after the last one are
+// read one by one.  The order in which f sees the elements is unspecified.
+template <class T, int U, class Fn>
+__device__ __forceinline__ void block_for_each(const T *__restrict__ s, uint64_t cnt, Fn f) {
+    static_assert(sizeof(T) == 4 || sizeof(T) == 8, "4- or 8-byte elements");
+    constexpr int V = 16 / (int)sizeof(T);
+    uint64_t head = ((16u - ((uint32_t)(uintptr_t)s & 15u)) & 15u) / sizeof(T);
+    if (head > cnt) head = cnt;
+    const uint64_t nvec = (cnt - head) / V, tail = head + nvec * V;
+    if (threadIdx.x < head) f(s[threadIdx.x], (uint64_t)threadIdx.x);
+    if (threadIdx.x < cnt - tail) f(s[tail + threadIdx.x], tail + threadIdx.x);
+    const uint4 *v = reinterpret_cast<const uint4 *>(s + head);
+    const uint64_t step = blockDim.x;
+    for (uint64_t q = threadIdx.x; q < nvec; q += U * step) {
+        uint4 x[U];
+#pragma unroll
+        for (int k = 0; k < U; k++) if (q + k * step < nvec) x[k] = __ldg(v + q + k * step);
+#pragma unroll
+        for (int k = 0; k < U; k++) {
+            if (q + k * step >= nvec) break;
+            const uint64_t i = head + (q + k * step) * V;
+            if constexpr (sizeof(T) == 4) { f(x[k].x, i); f(x[k].y, i + 1); f(x[k].z, i + 2); f(x[k].w, i + 3); }
+            else { f(make_uint2(x[k].x, x[k].y), i); f(make_uint2(x[k].z, x[k].w), i + 1); }
+        }
+    }
+}
+// Sort tiles: tile t of a domain holds its entries [t tile_len, (t+1) tile_len).  The per-tile counters of a domain are
+// stored tile-major ([tile][bin], one-level sort: few tiles, many bins, scanned by k_col_scan) or bin-major ([bin][tile],
+// coarse level: many tiles, 512 bins, scanned by k_bin_scan).
+__device__ __forceinline__ size_t tile_bin_index(int ws, int tile, int b, int tiles_per_ws, int nbins, bool bin_major) {
+    return bin_major ? ((size_t)ws * nbins + b) * tiles_per_ws + tile : ((size_t)ws * tiles_per_ws + tile) * nbins + b;
+}
+// Entries per coarse tile: the largest multiple of COARSE_CHUNK (4096) that still gives at least two waves of `resident`
+// k_coarse_scatter blocks over all domains (at least one chunk).
+constexpr int COARSE_PER_THREAD = 16, COARSE_CHUNK = COARSE_THREADS * COARSE_PER_THREAD;
+inline uint32_t coarse_tile_len(uint64_t e_dom, size_t n_dom, int resident) {
+    uint64_t t = e_dom * n_dom / (2 * (uint64_t)(resident > 0 ? resident : 1)) / COARSE_CHUNK * COARSE_CHUNK;
+    return (uint32_t)(t < (uint64_t)COARSE_CHUNK ? COARSE_CHUNK : t);
+}
 // `shift` > 0 bins by the high bits of the bucket key (coarse level of the two-level sort used for windows above 16 bits)
 static __global__ void __launch_bounds__(SORT_THREADS) k_tile_hist(const uint32_t *__restrict__ digits, uint64_t e_ws, int nbins, int shift,
-                                                            uint32_t *__restrict__ tile_hist, int tiles_per_ws) {
+                                                            uint32_t *__restrict__ tile_hist, int tiles_per_ws, uint32_t tile_len, bool bin_major) {
     extern __shared__ uint32_t sh[];
     int tile = blockIdx.x, ws = blockIdx.y;
     for (int b = threadIdx.x; b < nbins; b += blockDim.x) sh[b] = 0;
     __syncthreads();
-    uint64_t p0 = (uint64_t)tile * TILE, p1 = p0 + TILE < e_ws ? p0 + TILE : e_ws;
-    const uint32_t *d = digits + (size_t)ws * e_ws;
-    for (uint64_t p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
-        uint32_t code = d[p];
+    uint64_t p0 = (uint64_t)tile * tile_len, p1 = p0 + tile_len < e_ws ? p0 + tile_len : e_ws;
+    block_for_each<uint32_t, 4>(digits + (size_t)ws * e_ws + p0, p1 - p0, [&](uint32_t code, uint64_t) {
         if (code != DIGIT_ZERO) atomicAdd(&sh[(code & 0x7fffffffu) >> shift], 1u);
-    }
+    });
     __syncthreads();
-    uint32_t *o = tile_hist + ((size_t)ws * tiles_per_ws + tile) * nbins;
-    for (int b = threadIdx.x; b < nbins; b += blockDim.x) o[b] = sh[b];
+    for (int b = threadIdx.x; b < nbins; b += blockDim.x) tile_hist[tile_bin_index(ws, tile, b, tiles_per_ws, nbins, bin_major)] = sh[b];
 }
 // thread per (ws, bin): exclusive prefix over tiles -> tile_off, total -> sizes
 static __global__ void k_col_scan(const uint32_t *__restrict__ tile_hist, uint32_t *__restrict__ tile_off, uint32_t *__restrict__ sizes,
@@ -109,28 +152,109 @@ static __global__ void k_col_scan(const uint32_t *__restrict__ tile_hist, uint32
     }
     sizes[g] = run;
 }
-// KEYED (coarse level of the two-level sort): each entry is stored as {payload, bucket key}, so that k_fine_sort reads the
-// key with the entry instead of gathering it from the digits array (a random 4-byte read costs a 32-byte sector)
-template <bool KEYED>
-static __global__ void __launch_bounds__(SORT_THREADS) k_scatter(const uint32_t *__restrict__ digits, uint64_t e_ws, int nbins, int shift,
+// Coarse level (bin-major counters): block per (ws, bin), exclusive prefix of the bin's counters over the tiles ->
+// tile_off (same layout), total -> sizes.  The block scans COARSE_THREADS x 4 counters per step with warp shuffles.
+static __global__ void __launch_bounds__(COARSE_THREADS) k_bin_scan(const uint32_t *__restrict__ tile_hist, uint32_t *__restrict__ tile_off,
+                                                                    uint32_t *__restrict__ sizes, int tiles_per_ws) {
+    __shared__ uint32_t wsum[COARSE_THREADS / 32];
+    const uint32_t *in = tile_hist + (size_t)blockIdx.x * tiles_per_ws;
+    uint32_t *out = tile_off + (size_t)blockIdx.x * tiles_per_ws;
+    uint32_t run = 0;
+    for (int base = 0; base < tiles_per_ws; base += COARSE_THREADS * 4) {
+        const int t0 = base + threadIdx.x * 4;
+        uint32_t v[4], s = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) { v[k] = t0 + k < tiles_per_ws ? in[t0 + k] : 0; s += v[k]; }
+        uint32_t inc = s;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if ((threadIdx.x & 31) >= (unsigned)o) inc += t; }
+        if ((threadIdx.x & 31) == 31) wsum[threadIdx.x >> 5] = inc;
+        __syncthreads();
+        uint32_t before = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < COARSE_THREADS / 32; w++) { const uint32_t x = wsum[w]; before += w < (int)(threadIdx.x >> 5) ? x : 0; total += x; }
+        uint32_t ex = run + before + inc - s;
+#pragma unroll
+        for (int k = 0; k < 4; k++) { if (t0 + k < tiles_per_ws) out[t0 + k] = ex; ex += v[k]; }
+        run += total;
+        __syncthreads();                               // wsum is rewritten by the next step
+    }
+    if (threadIdx.x == 0) sizes[blockIdx.x] = run;
+}
+// one-level sort: entries go straight from the digits to their bucket's cursor
+static __global__ void __launch_bounds__(SORT_THREADS) k_scatter(const uint32_t *__restrict__ digits, uint64_t e_ws, int nbins,
                                                           const uint32_t *__restrict__ tile_off, const uint32_t *__restrict__ bucket_off,
-                                                          void *__restrict__ sorted, int tiles_per_ws) {
+                                                          uint32_t *__restrict__ sorted, int tiles_per_ws, uint32_t tile_len) {
     extern __shared__ uint32_t sh[];
     int tile = blockIdx.x, ws = blockIdx.y;
-    const uint32_t *to = tile_off + ((size_t)ws * tiles_per_ws + tile) * nbins;
     const uint32_t *bo = bucket_off + (size_t)ws * nbins;
-    for (int b = threadIdx.x; b < nbins; b += blockDim.x) sh[b] = bo[b] + to[b];
+    for (int b = threadIdx.x; b < nbins; b += blockDim.x) sh[b] = bo[b] + tile_off[tile_bin_index(ws, tile, b, tiles_per_ws, nbins, false)];
     __syncthreads();
-    uint64_t p0 = (uint64_t)tile * TILE, p1 = p0 + TILE < e_ws ? p0 + TILE : e_ws;
+    uint64_t p0 = (uint64_t)tile * tile_len, p1 = p0 + tile_len < e_ws ? p0 + tile_len : e_ws;
+    block_for_each<uint32_t, 4>(digits + (size_t)ws * e_ws + p0, p1 - p0, [&](uint32_t code, uint64_t i) {
+        if (code != DIGIT_ZERO) sorted[atomicAdd(&sh[code & 0x7fffffffu], 1u)] = (uint32_t)(p0 + i) | (code & 0x80000000u);
+    });
+}
+// Coarse level of the two-level sort: each entry is stored as {payload, bucket key}, so that k_fine_sort reads the key
+// with the entry instead of gathering it from the digits array (a random 4-byte read costs a 32-byte sector).  A tile is
+// taken in chunks of COARSE_CHUNK entries (16 loads in flight per thread); each chunk is first grouped by coarse bin in
+// shared memory, so that the global stores are runs of consecutive addresses per bin instead of one 8-byte store per
+// sector (8 entries per bin and chunk on average at 512 bins).
+constexpr int COARSE_BINS = 512;
+static __global__ void __launch_bounds__(COARSE_THREADS) k_coarse_scatter(const uint32_t *__restrict__ digits, uint64_t e_ws, int shift,
+                                                                          const uint32_t *__restrict__ tile_off, const uint32_t *__restrict__ bin_off,
+                                                                          uint2 *__restrict__ sorted, int tiles_per_ws, uint32_t tile_len) {
+    __shared__ uint2 stage[COARSE_CHUNK];
+    __shared__ uint32_t cur[COARSE_BINS], cnt[COARSE_BINS], loff[COARSE_BINS], wsum[COARSE_THREADS / 32 + 1];
+    const int tile = blockIdx.x, ws = blockIdx.y;
+    for (int b = threadIdx.x; b < COARSE_BINS; b += COARSE_THREADS)
+        cur[b] = bin_off[(size_t)ws * COARSE_BINS + b] + tile_off[tile_bin_index(ws, tile, b, tiles_per_ws, COARSE_BINS, true)];
+    const uint64_t p0 = (uint64_t)tile * tile_len, p1 = p0 + tile_len < e_ws ? p0 + tile_len : e_ws;
     const uint32_t *d = digits + (size_t)ws * e_ws;
-    for (uint64_t p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
-        uint32_t code = d[p];
-        if (code != DIGIT_ZERO) {
-            uint32_t pos = atomicAdd(&sh[(code & 0x7fffffffu) >> shift], 1u);
-            const uint32_t entry = (uint32_t)p | (code & 0x80000000u);
-            if (KEYED) reinterpret_cast<uint2 *>(sorted)[pos] = make_uint2(entry, code & 0x7fffffffu);
-            else reinterpret_cast<uint32_t *>(sorted)[pos] = entry;
+    for (uint64_t c0 = p0; c0 < p1; c0 += COARSE_CHUNK) {
+        for (int b = threadIdx.x; b < COARSE_BINS; b += COARSE_THREADS) cnt[b] = 0;
+        __syncthreads();
+        uint32_t code[COARSE_PER_THREAD], rank[COARSE_PER_THREAD];
+#pragma unroll
+        for (int k = 0; k < COARSE_PER_THREAD; k++) {
+            const uint64_t p = c0 + threadIdx.x + k * COARSE_THREADS;
+            code[k] = p < p1 ? __ldg(d + p) : DIGIT_ZERO;
         }
+#pragma unroll
+        for (int k = 0; k < COARSE_PER_THREAD; k++)
+            if (code[k] != DIGIT_ZERO) rank[k] = atomicAdd(&cnt[(code[k] & 0x7fffffffu) >> shift], 1u);
+        __syncthreads();
+        {   // exclusive scan of the 512 chunk counters, two per thread
+            const uint32_t a = cnt[2 * threadIdx.x], b = cnt[2 * threadIdx.x + 1], s = a + b;
+            uint32_t inc = s;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if ((threadIdx.x & 31) >= (unsigned)o) inc += t; }
+            if ((threadIdx.x & 31) == 31) wsum[threadIdx.x >> 5] = inc;
+            __syncthreads();
+            uint32_t before = 0;
+            for (int w = 0; w < (int)(threadIdx.x >> 5); w++) before += wsum[w];
+            const uint32_t ex = before + inc - s;
+            loff[2 * threadIdx.x] = ex;
+            loff[2 * threadIdx.x + 1] = ex + a;
+            if (threadIdx.x == COARSE_THREADS - 1) wsum[COARSE_THREADS / 32] = ex + s;     // entries of the chunk
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < COARSE_PER_THREAD; k++)
+            if (code[k] != DIGIT_ZERO) {
+                const uint32_t key = code[k] & 0x7fffffffu;
+                const uint32_t entry = (uint32_t)(c0 + threadIdx.x + k * COARSE_THREADS) | (code[k] & 0x80000000u);
+                stage[loff[key >> shift] + rank[k]] = make_uint2(entry, key);
+            }
+        __syncthreads();
+        const uint32_t total = wsum[COARSE_THREADS / 32];
+        for (uint32_t j = threadIdx.x; j < total; j += COARSE_THREADS) {
+            const uint2 e = stage[j];
+            const uint32_t b = e.y >> shift;
+            sorted[cur[b] + j - loff[b]] = e;
+        }
+        __syncthreads();
+        for (int b = threadIdx.x; b < COARSE_BINS; b += COARSE_THREADS) cur[b] += cnt[b];
     }
 }
 
@@ -138,20 +262,28 @@ static __global__ void __launch_bounds__(SORT_THREADS) k_scatter(const uint32_t 
 // One block per (coarse bin, domain): the entries of the coarse bin (already contiguous) are counted by the low `low`
 // bits of their key in shared memory, the counts are scanned, and the entries are scattered to their final places.
 // Writes bucket sizes and bucket offsets directly (no global scan needed); the bucket key of an entry comes with it from
-// k_scatter<true>, so both passes read the coarse bin contiguously.
-static __global__ void __launch_bounds__(1024) k_fine_sort(const uint2 *__restrict__ coarse_sorted, const uint32_t *__restrict__ coarse_off,
+// k_coarse_scatter, so every pass reads the coarse bin contiguously, with 16-byte loads of two entries and four loads in
+// flight per thread.
+// The scatter goes to a FINE_STAGE-entry window of shared memory that is then copied out with coalesced stores: one
+// 4-byte store per entry straight to HBM would leave hundreds of blocks' whole output regions as partly written sectors in
+// L2 at once.  A bin whose output is larger than the window is scattered in segments of consecutive buckets that fit it,
+// one more pass over the bin per segment; a bucket larger than the window, or a bin of more than FINE_MAX_SEGMENTS
+// windows, is scattered straight to HBM instead.
+constexpr int FINE_STAGE = 25 * 1024, FINE_MAX_SEGMENTS = 4;      // 100 KB of shared memory: two blocks per SM
+static __global__ void __launch_bounds__(1024, 2) k_fine_sort(const uint2 *__restrict__ coarse_sorted, const uint32_t *__restrict__ coarse_off,
                                                           int n_coarse, int low,
                                                           uint32_t *__restrict__ sizes, uint32_t *__restrict__ bucket_off, uint32_t *__restrict__ sorted) {
-    __shared__ uint32_t hist[1024];
+    extern __shared__ uint32_t stage[];                  // FINE_STAGE entries
+    __shared__ uint32_t hist[1024], off[1025];
     __shared__ uint32_t wsum[32];
     const int cb = blockIdx.x, dom = blockIdx.y, g = dom * n_coarse + cb;
-    const uint32_t r0 = coarse_off[g], r1 = coarse_off[g + 1], fmask = (1u << low) - 1u;
+    const uint32_t r0 = coarse_off[g], r1 = coarse_off[g + 1], nb = 1u << low, fmask = nb - 1u;
     hist[threadIdx.x] = 0;
     __syncthreads();
-    for (uint32_t i = r0 + threadIdx.x; i < r1; i += blockDim.x) atomicAdd(&hist[coarse_sorted[i].y & fmask], 1u);
+    block_for_each<uint2, 4>(coarse_sorted + r0, r1 - r0, [&](uint2 e, uint64_t) { atomicAdd(&hist[e.y & fmask], 1u); });
     __syncthreads();
     // exclusive scan of the (<= 1024) counters: one per thread
-    uint32_t v = threadIdx.x < (1u << low) ? hist[threadIdx.x] : 0, inc = v;
+    uint32_t v = threadIdx.x < nb ? hist[threadIdx.x] : 0, inc = v;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if ((threadIdx.x & 31) >= (unsigned)o) inc += t; }
     if ((threadIdx.x & 31) == 31) wsum[threadIdx.x >> 5] = inc;
@@ -165,17 +297,39 @@ static __global__ void __launch_bounds__(1024) k_fine_sort(const uint2 *__restri
     __syncthreads();
     uint32_t excl = inc - v + wsum[threadIdx.x >> 5];
     __syncthreads();
-    if (threadIdx.x < (1u << low)) {
+    if (threadIdx.x < nb) {
         size_t b = ((size_t)g << low) + threadIdx.x;
         sizes[b] = v;
         bucket_off[b] = r0 + excl;
         hist[threadIdx.x] = r0 + excl;           // becomes the scatter cursor
+        off[threadIdx.x] = excl;                 // bucket start inside the bin
+        if (threadIdx.x == nb - 1) off[nb] = excl + v;
     }
     if (cb == n_coarse - 1 && dom == (int)gridDim.y - 1 && threadIdx.x == 0) bucket_off[((size_t)g + 1) << low] = r1;
     __syncthreads();
-    for (uint32_t i = r0 + threadIdx.x; i < r1; i += blockDim.x) {
-        const uint2 e = coarse_sorted[i];
-        sorted[atomicAdd(&hist[e.y & fmask], 1u)] = e.x;
+    const uint32_t total = r1 - r0;
+    if (total > (uint32_t)FINE_MAX_SEGMENTS * FINE_STAGE) {
+        block_for_each<uint2, 4>(coarse_sorted + r0, total, [&](uint2 e, uint64_t) { sorted[atomicAdd(&hist[e.y & fmask], 1u)] = e.x; });
+        return;
+    }
+    for (uint32_t lo = 0; lo < nb;) {                    // segment [lo, hi) of buckets, the same on every thread
+        const uint32_t base = off[lo];
+        const int fit = __syncthreads_count(threadIdx.x >= lo && threadIdx.x < nb && off[threadIdx.x + 1] - base <= (uint32_t)FINE_STAGE);
+        const uint32_t hi = lo + (fit > 0 ? (uint32_t)fit : 1u);
+        const bool direct = fit == 0;                    // bucket lo alone is larger than the window
+        block_for_each<uint2, 2>(coarse_sorted + r0, total, [&](uint2 e, uint64_t) {     // 2 loads in flight: 32 registers
+            const uint32_t k = e.y & fmask;
+            if (k >= lo && k < hi) {
+                const uint32_t p = atomicAdd(&hist[k], 1u);
+                if (direct) sorted[p] = e.x;
+                else stage[p - r0 - base] = e.x;
+            }
+        });
+        __syncthreads();
+        if (!direct)
+            for (uint32_t j = threadIdx.x, m = off[hi] - base; j < m; j += blockDim.x) sorted[r0 + base + j] = stage[j];
+        __syncthreads();
+        lo = hi;
     }
 }
 

@@ -28,7 +28,18 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
     const uint64_t e_dom = tables ? (uint64_t)n * W : (uint64_t)n;
     const size_t E = (size_t)n * W * batch;
     if (E >= ((size_t)1 << 31)) { zk_set_error("MSM too large for 31-bit entry payloads (n*W*batch = %zu)", E); return ZK_ERR_INVALID; }
-    const int tiles = (int)((e_dom + TILE - 1) / TILE);
+    // sort tiles: fixed TILE for the one-level sort (c <= 16, up to 128 KB of shared counters per block); the coarse level of
+    // the two-level sort (c > 16, 2 KB of counters) uses small tiles, enough of them to fill every SM twice
+    const bool two_level = c > 16;
+    const int low = two_level ? (c - 1) - 9 : 0, sort_bins = two_level ? 512 : nbins;
+    size_t smem = (size_t)sort_bins * 4;
+    uint32_t tile_len = TILE;
+    if (two_level) {
+        int per_sm = 0;
+        ZK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_coarse_scatter, COARSE_THREADS, 0));
+        tile_len = coarse_tile_len(e_dom, n_dom, per_sm * ctx->sm_count);
+    }
+    const int tiles = (int)((e_dom + tile_len - 1) / tile_len);
     const size_t NB = n_dom * nbins;
     // tasks: round(size_b / task_len) >= 1 per non-empty bucket, summed <= total/task_len + NB (k_pick_task_len), and
     // total/task_len <= E/TASK_LEN_MAX + two waves of k_accumulate (sm_count x 384 resident tasks; 1024 per SM leaves margin)
@@ -58,32 +69,30 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
     }
     // 2. counting sort per domain.  Up to 16-bit windows the 2^(c-1) bucket counters fit in shared memory (one level);
     //    wider windows sort by the high 9 key bits first and finish each coarse bin in shared memory (k_fine_sort).
-    const bool two_level = c > 16;
-    const int low = two_level ? (c - 1) - 9 : 0, sort_bins = two_level ? 512 : nbins;
     const size_t SB = n_dom * (size_t)sort_bins;
-    size_t smem = (size_t)sort_bins * 4;
     if (smem > 48 * 1024) {
         ZK_CUDA(cudaFuncSetAttribute(k_tile_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ZK_CUDA(cudaFuncSetAttribute(k_scatter<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ZK_CUDA(cudaFuncSetAttribute(k_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 gs((unsigned)tiles, (unsigned)n_dom);
     if (!two_level) {
-        k_tile_hist<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, nbins, 0, ctx->tile_hist.as<uint32_t>(), tiles);
+        k_tile_hist<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, nbins, 0, ctx->tile_hist.as<uint32_t>(), tiles, tile_len, false);
         k_col_scan<<<(unsigned)((NB + 255) / 256), 256, 0, st>>>(ctx->tile_hist.as<uint32_t>(), ctx->tile_off.as<uint32_t>(), ctx->sizes.as<uint32_t>(),
                                                                 nbins, tiles, (int)n_dom);
         exclusive_scan<false>(ctx->sizes.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(), NB, ctx->scan_scratch.as<uint32_t>(), st);
-        k_scatter<false><<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, nbins, 0, ctx->tile_off.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(),
-                                                  ctx->sorted.as<uint32_t>(), tiles);
+        k_scatter<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, nbins, ctx->tile_off.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(),
+                                                  ctx->sorted.as<uint32_t>(), tiles, tile_len);
     } else {
-        ZK_TRY(ctx->sorted2.reserve(E * sizeof(uint2)));           // {entry, bucket key} per entry (k_scatter<true>)
+        ZK_TRY(ctx->sorted2.reserve(E * sizeof(uint2)));           // {entry, bucket key} per entry (k_coarse_scatter)
         ZK_TRY(ctx->coarse_off.reserve((SB + 1) * 4)); ZK_TRY(ctx->coarse_sizes.reserve((SB + 1) * 4));
-        k_tile_hist<<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, sort_bins, low, ctx->tile_hist.as<uint32_t>(), tiles);
-        k_col_scan<<<(unsigned)((SB + 255) / 256), 256, 0, st>>>(ctx->tile_hist.as<uint32_t>(), ctx->tile_off.as<uint32_t>(), ctx->coarse_sizes.as<uint32_t>(),
-                                                                sort_bins, tiles, (int)n_dom);
+        // per-tile counters bin-major ([domain][bin][tile]): k_bin_scan reads each bin's counters contiguously
+        k_tile_hist<<<gs, COARSE_THREADS, smem, st>>>(digits, e_dom, sort_bins, low, ctx->tile_hist.as<uint32_t>(), tiles, tile_len, true);
+        k_bin_scan<<<(unsigned)SB, COARSE_THREADS, 0, st>>>(ctx->tile_hist.as<uint32_t>(), ctx->tile_off.as<uint32_t>(), ctx->coarse_sizes.as<uint32_t>(), tiles);
         exclusive_scan<false>(ctx->coarse_sizes.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(), SB, ctx->scan_scratch.as<uint32_t>(), st);
-        k_scatter<true><<<gs, SORT_THREADS, smem, st>>>(digits, e_dom, sort_bins, low, ctx->tile_off.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(),
-                                                        ctx->sorted2.p, tiles);
-        k_fine_sort<<<dim3(512, (unsigned)n_dom), 1024, 0, st>>>(ctx->sorted2.as<uint2>(), ctx->coarse_off.as<uint32_t>(), 512, low,
+        k_coarse_scatter<<<gs, COARSE_THREADS, 0, st>>>(digits, e_dom, low, ctx->tile_off.as<uint32_t>(), ctx->coarse_off.as<uint32_t>(),
+                                                        ctx->sorted2.as<uint2>(), tiles, tile_len);
+        ZK_CUDA(cudaFuncSetAttribute(k_fine_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, FINE_STAGE * 4));
+        k_fine_sort<<<dim3(512, (unsigned)n_dom), 1024, FINE_STAGE * 4, st>>>(ctx->sorted2.as<uint2>(), ctx->coarse_off.as<uint32_t>(), 512, low,
                                                                  ctx->sizes.as<uint32_t>(), ctx->bucket_off.as<uint32_t>(), ctx->sorted.as<uint32_t>());
     }
     // 2b. batched-affine rounds (msm_batchaff.cuh): each round halves every bucket at ~6.4 products per addition instead of the 10
