@@ -308,6 +308,39 @@ int zk_elgamal_decrypt_batch(zk_ctx *ctx, size_t n, const uint8_t *dks, const ui
 /* the same with device pointers (d_values 4-byte aligned); asynchronous on the context's stream */
 int zk_elgamal_decrypt_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_dks, const uint8_t *d_cts, const uint8_t *d_pending,
                                     uint32_t *d_values, uint8_t *d_status);
+/* ---- confidential-transfer balance updates of one block (what modules/encrypted-balances runs around each proof) ------
+ * rollover + sub_enc_balance + add_pending_transfer (modules/encrypted-balances/src/lib.rs:25-96, 133-222) for n_tx
+ * transactions, in order, over a table of n_accounts accounts.
+ * balances / pendings: n_accounts * 64 B (Ciphertext: left | right); acct_flags[a]: bit 0 balance present, bit 1 pending
+ * present, bit 2 rollover due (last_rollover < current_epoch, worked out by the caller).  An account is rolled over at its
+ * first touch by any transaction, if due: balance = (balance or zero) + (pending or zero), present; pending absent.
+ * sender / recipient: n_tx account indices; tx_points: n_tx * 128 B, amount_sender | amount_recipient | fee_sender |
+ * randomness; applied[k]: 1 when transaction k passed its checks (the proof verdict), else 0.
+ * balance_sender[k]: 64 B, the sender's balance that verify_confidential_proof reads (Ciphertext::zero() when absent).
+ * balance_after[k]: 64 B, the sender's balance after the transaction (the ConfidentialTransfer event); written for applied
+ *   transactions only, the other entries are left as they are.
+ * tx_status[k]: 0 applied (balance -= (amount_sender + fee_sender, 2 randomness), an absent balance staying absent;
+ *   pending(recipient) += (amount_recipient, randomness)); 1 not applied (applied[k] = 0); 2 a transaction point fails
+ *   Point::read + as_prime_order (not applied: the verifier rejects the same point); 3 sender or recipient >= n_accounts
+ *   (not applied, and it touches no account).  When several apply, 3 comes before 2 and 2 before 1.
+ * new_balances / new_pendings / new_flags: the state after the block.  Untouched accounts are copied through byte for byte;
+ *   a touched account's absent ciphertexts are 64 zero bytes, its flags keep bits 3-7, and bit 2 is cleared.
+ * ZK_ERR_DECODE when a touched account's stored ciphertext (balance or pending, when present) fails Ciphertext::read;
+ *   zk_last_error names the lowest such account, and the outputs are undefined.  ZK_ERR_INVALID for a NULL ctx, for a NULL
+ *   account array when n_accounts > 0 or transaction array when n_tx > 0, and for n_accounts or n_tx above 2^22.  n_tx = 0
+ *   gives the state back unchanged. */
+int zk_balances_confidential_block(zk_ctx *ctx, size_t n_accounts, const uint8_t *balances, const uint8_t *pendings,
+                                   const uint8_t *acct_flags, size_t n_tx, const uint32_t *sender, const uint32_t *recipient,
+                                   const uint8_t *tx_points, const uint8_t *applied, uint8_t *balance_sender, uint8_t *balance_after,
+                                   uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags);
+/* the same with device pointers (d_sender / d_recipient 4-byte aligned); asynchronous on the context's stream.  A touched
+ * account that fails to decode is reported by the next zk_ctx_sync (or the next call that reports the context's pending
+ * device errors) as ZK_ERR_DECODE, with the account named in zk_last_error */
+int zk_balances_confidential_block_device(zk_ctx *ctx, size_t n_accounts, const uint8_t *d_balances, const uint8_t *d_pendings,
+                                          const uint8_t *d_acct_flags, size_t n_tx, const uint32_t *d_sender,
+                                          const uint32_t *d_recipient, const uint8_t *d_tx_points, const uint8_t *d_applied,
+                                          uint8_t *d_balance_sender, uint8_t *d_balance_after, uint8_t *d_tx_status,
+                                          uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

@@ -38,7 +38,7 @@ extern "C" int zk_ctx_create(int device, void *stream, zk_ctx **out) {
     cudaDeviceProp prop;
     ZK_CUDA(cudaGetDeviceProperties(&prop, device));
     c->sm_count = prop.multiProcessorCount;
-    ZK_CUDA(cudaMalloc(&c->d_err, 32 * sizeof(int)));       // [0..1] error flags, [8..9] task length / heavy-bucket count, [10..17] work counters
+    ZK_CUDA(cudaMalloc(&c->d_err, 32 * sizeof(int)));       // [0..1] error flags, [2] failing account of zk_balances_confidential_block, [8..9] task length / heavy-bucket count, [10..17] work counters
     ZK_CUDA(cudaMemsetAsync(c->d_err, 0, 32 * sizeof(int), c->stream));
     c->h_pinned_cap = 1 << 20;
     ZK_CUDA(cudaMallocHost(&c->h_pinned, c->h_pinned_cap));
@@ -57,7 +57,7 @@ extern "C" void zk_ctx_destroy(zk_ctx *c) {
                       &c->stage_c, &c->ntt_tmp, &c->g_a, &c->g_b, &c->g_c, &c->g_h, &c->g_scal, &c->g_misc,
                       &c->aff_pts0, &c->aff_pts1, &c->aff_scratch, &c->aff_off0, &c->aff_off1, &c->aff_sizes0, &c->aff_sizes1, &c->aff_srcs, &c->aff_tot, &c->red_rows, &c->g_scal2, &c->g_scal3, &c->sorted2, &c->coarse_off, &c->coarse_sizes, &c->task_order, &c->len_hist, &c->heavy_list, &c->red_tmp,
                       &c->v_pts, &c->v_stat, &c->v_coef, &c->v_f, &c->v_part, &c->v_io, &c->v_jj,
-                      &c->eg_table, &c->eg_index, &c->jm};
+                      &c->eg_table, &c->eg_index, &c->jm, &c->bal, &c->bal_io};
     for (DevBuf *b : bufs) b->release();
     for (NttSlot &sl : c->ntt_slots) { sl.w.release(); sl.g.release(); sl.gi.release(); sl.consts.release(); }
     if (c->tail) { cudaStreamSynchronize(c->tail); cudaStreamDestroy(c->tail); cudaEventDestroy(c->ev_front); cudaEventDestroy(c->ev_tail); }
@@ -81,12 +81,16 @@ extern "C" int zk_ctx_sync(zk_ctx *c) { ZK_TRY(zk_use_device(c)); return zk_chec
 extern "C" void *zk_ctx_stream(zk_ctx *c) { return (void *)c->stream; }
 
 int zk_check_err_flag(zk_ctx *ctx) {
-    int e[2] = {0, 0};
+    int e[3] = {0, 0, 0};
     ZK_CUDA(cudaMemcpyAsync(e, ctx->d_err, sizeof(e), cudaMemcpyDeviceToHost, ctx->stream));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (e[0] || e[1]) {
-        ZK_CUDA(cudaMemsetAsync(ctx->d_err, 0, 2 * sizeof(int), ctx->stream));
+    if (e[0] || e[1] || e[ZK_ERR_SLOT_ACCOUNT]) {
+        ZK_CUDA(cudaMemsetAsync(ctx->d_err, 0, sizeof(e), ctx->stream));
         if (e[0]) { zk_set_error("scalar not canonical (>= r)"); return ZK_ERR_NOT_CANONICAL; }
+        if (e[ZK_ERR_SLOT_ACCOUNT]) {
+            zk_set_error("account %u: a stored ciphertext fails Ciphertext::read", ~(uint32_t)e[ZK_ERR_SLOT_ACCOUNT]);
+            return ZK_ERR_DECODE;
+        }
         zk_set_error("point decoding failed (GroupDecodingError %d)", e[1]);
         return e[1] == zkcodec::DEC_INFINITY ? ZK_ERR_UNEXPECTED_IDENTITY : ZK_ERR_DECODE;
     }

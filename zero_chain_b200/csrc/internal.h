@@ -74,6 +74,7 @@ struct zk_ctx {
     // zk_elgamal_decrypt_batch (elgamal.cu): the encodings of i P_G for i < 10^6 and their index, built by the first call
     DevBuf eg_table, eg_index;
     bool eg_ready = false;
+    DevBuf bal, bal_io;            // zk_balances_confidential_block (balances.cu): workspace, and the host form's staging
     DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;
@@ -119,6 +120,8 @@ int zk_fr_quotient(zk_ctx *ctx, const void *d_abc, unsigned log_m, size_t batch,
 int zk_fr_into_repr(zk_ctx *ctx, const void *d_h, unsigned log_m, size_t n_out, size_t n_total, size_t batch, void *d_scal);
 int zk_fr_blinding_terms(zk_ctx *ctx, const void *d_r, const void *d_s, size_t batch, void *d_out);
 int zk_check_err_flag(zk_ctx *ctx);
+// d_err[ZK_ERR_SLOT_ACCOUNT]: ~(the lowest account whose stored ciphertext failed to read) in zk_balances_confidential_block, 0: none
+constexpr int ZK_ERR_SLOT_ACCOUNT = 2;
 // lane-parallel verifier kernels (pairing_lanes.cu)
 void zk_launch_miller_lanes(cudaStream_t st, size_t n, const void *a, const void *acc, const void *c, const void *coef_b, const void *gamma, int gamma_inf,
                             const void *delta, int delta_inf, const uint8_t *status, void *f);

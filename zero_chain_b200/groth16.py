@@ -546,6 +546,124 @@ def elgamal_decrypt_device(ctx: Context, n: int, d_dks_ptr: int, d_cts_ptr: int,
                                                    C.c_void_p(d_status_ptr)))
 
 
+# ---- confidential-transfer balance updates of one block (modules/encrypted-balances/src/lib.rs:25-96, 133-222) ----------
+# account flags and zk_balances_confidential_block statuses
+ACCOUNT_BALANCE, ACCOUNT_PENDING, ACCOUNT_DUE = 1, 2, 4
+BLOCK_APPLIED, BLOCK_NOT_APPLIED, BLOCK_BAD_POINT, BLOCK_BAD_INDEX = 0, 1, 2, 3
+
+
+def confidential_block(ctx: Context, balances, pendings, flags, sender, recipient, tx_points, applied):
+    """rollover + sub_enc_balance + add_pending_transfer over a block, in order (zk_balances_confidential_block).
+    balances / pendings: 64 bytes per account; flags: one ACCOUNT_* byte per account; sender / recipient: account indices;
+    tx_points: 128 bytes per transaction (amount_sender | amount_recipient | fee_sender | randomness); applied: one byte per
+    transaction.  Returns (balance_sender, balance_after, status, new_balances, new_pendings, new_flags) as bytes;
+    balance_after is zero for transactions that are not applied.  Raises SynthesisError(ZK_ERR_DECODE) naming the account
+    when a touched account's stored ciphertext does not read."""
+    n_acct, n_tx = len(flags), len(sender)
+    bal, pend, fl, tp, ap = (_cat(balances, 64), _cat(pendings, 64), bytes(flags), _cat(tx_points, 128), bytes(applied))
+    assert len(bal) == len(pend) == 64 * n_acct and len(recipient) == n_tx and len(tp) == 128 * n_tx and len(ap) == n_tx
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    idx = lambda v: np.ascontiguousarray(v, np.uint32) if n_tx else np.zeros(1, np.uint32)
+    bs, ba = np.zeros(max(64 * n_tx, 1), np.uint8), np.zeros(max(64 * n_tx, 1), np.uint8)
+    st = np.zeros(max(n_tx, 1), np.uint8)
+    nb, npd = np.zeros(max(64 * n_acct, 1), np.uint8), np.zeros(max(64 * n_acct, 1), np.uint8)
+    nf = np.zeros(max(n_acct, 1), np.uint8)
+    _ck(_lib.lib().zk_balances_confidential_block(ctx._h, n_acct, _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n_tx, _p(idx(sender)),
+                                                  _p(idx(recipient)), _p(buf(tp)), _p(buf(ap)), _p(bs), _p(ba), _p(st), _p(nb), _p(npd), _p(nf)))
+    return (bs[:64 * n_tx].tobytes(), ba[:64 * n_tx].tobytes(), st[:n_tx].tobytes(), nb[:64 * n_acct].tobytes(),
+            npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes())
+
+
+def confidential_block_device(ctx: Context, n_accounts: int, d_balances_ptr: int, d_pendings_ptr: int, d_flags_ptr: int, n_tx: int,
+                              d_sender_ptr: int, d_recipient_ptr: int, d_tx_points_ptr: int, d_applied_ptr: int,
+                              d_balance_sender_ptr: int, d_balance_after_ptr: int, d_status_ptr: int, d_new_balances_ptr: int,
+                              d_new_pendings_ptr: int, d_new_flags_ptr: int):
+    """The same on device pointers (d_sender / d_recipient: uint32), asynchronous on the context's stream; ctx.sync()
+    raises SynthesisError(ZK_ERR_DECODE) naming a touched account whose stored ciphertext did not read.  Only the applied
+    transactions' entries of d_balance_after are written."""
+    v = lambda x: C.c_void_p(x) if x else None
+    _ck(_lib.lib().zk_balances_confidential_block_device(ctx._h, n_accounts, v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr), n_tx,
+                                                         v(d_sender_ptr), v(d_recipient_ptr), v(d_tx_points_ptr), v(d_applied_ptr),
+                                                         v(d_balance_sender_ptr), v(d_balance_after_ptr), v(d_status_ptr),
+                                                         v(d_new_balances_ptr), v(d_new_pendings_ptr), v(d_new_flags_ptr)))
+
+
+class ConfidentialTx:
+    """One confidential_transfer extrinsic (lib.rs:25-35) with its accounts as indices into the block's account table."""
+
+    def __init__(self, sender: int, recipient: int, address_sender, address_recipient, amount_sender, amount_recipient, fee_sender,
+                 randomness, rvk, g_epoch, nonce):
+        self.sender, self.recipient = sender, recipient
+        self.address_sender, self.address_recipient = _pt32(address_sender), _pt32(address_recipient)
+        self.amount_sender, self.amount_recipient = _pt32(amount_sender), _pt32(amount_recipient)
+        self.fee_sender, self.randomness = _pt32(fee_sender), _pt32(randomness)
+        self.rvk, self.g_epoch, self.nonce = _pt32(rvk), _pt32(g_epoch), _pt32(nonce)
+
+    def points(self) -> bytes:
+        return self.amount_sender + self.amount_recipient + self.fee_sender + self.randomness
+
+
+def import_confidential_block(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, proofs):
+    """Verify and apply a block of confidential transfers the way the runtime does, one extrinsic after another, with the
+    state and the proofs of the whole block on the device.  accounts = (balances, pendings, flags) as confidential_block
+    takes them; txs: ConfidentialTx list; proofs: 192 bytes each.
+
+    A proof is checked against the sender's balance as it stands at its transaction, which depends on which of the
+    sender's earlier transactions passed.  So every transaction starts as applied, and each round computes the balances
+    (confidential_block), verifies the undecided transactions (verify_proofs_with_points), and decides, in each sender's
+    chain, the transactions up to and including the first whose verdict is not 1: their balances were exact.  The rest
+    waits for the next round.  A block takes 1 + (the most failures in one sender's chain) rounds at most; a block with
+    no failures takes one.
+
+    Returns (verdicts, (new_balances, new_pendings, new_flags), balance_after, rounds): the reference's verdict per
+    transaction (1 passes; the other values as verify_proofs_with_points).  Raises ValueError for an account index out of
+    range, SynthesisError(ZK_ERR_DECODE) for a touched account whose stored ciphertext does not read."""
+    balances, pendings, flags = accounts
+    n = len(txs)
+    if any(not (0 <= t.sender < len(flags) and 0 <= t.recipient < len(flags)) for t in txs):
+        raise ValueError("import_confidential_block: account index out of range")
+    proofs = _cat(proofs, 192)
+    assert len(proofs) == 192 * n
+    sender = np.array([t.sender for t in txs], np.uint32)
+    recipient = np.array([t.recipient for t in txs], np.uint32)
+    # every transaction's public-input points in confidential_points order; columns 6-7 (balance_sender) are filled per round
+    inputs = np.frombuffer(b"".join(t.address_sender + t.address_recipient + t.amount_sender + t.amount_recipient + t.randomness +
+                                    t.fee_sender + bytes(64) + t.rvk + t.g_epoch + t.nonce for t in txs), np.uint8)
+    inputs = inputs.reshape(n, CONFIDENTIAL_POINTS, 32).copy()
+    tx_points = inputs[:, [2, 3, 5, 4], :].tobytes()          # amount_sender | amount_recipient | fee_sender | randomness
+    proof_rows = np.frombuffer(proofs, np.uint8).reshape(n, 192)
+    verdicts = np.full(n, -1, np.int16)                      # -1: undecided
+    chains = None
+    rounds = 0
+    while True:
+        out = confidential_block(ctx, balances, pendings, flags, sender, recipient, tx_points,
+                                 ((verdicts == -1) | (verdicts == 1)).astype(np.uint8).tobytes())
+        undecided = np.flatnonzero(verdicts == -1)
+        if not len(undecided):
+            break
+        rounds += 1
+        inputs[:, 6:8, :] = np.frombuffer(out[0], np.uint8).reshape(n, 2, 32)
+        sel = slice(None) if len(undecided) == n else undecided
+        got = np.array(verify_proofs_with_points(pvk, proof_rows[sel].tobytes(), inputs[sel].tobytes(), CONFIDENTIAL_POINTS), np.int16)
+        if (got == 1).all():
+            verdicts[undecided] = 1
+            break                   # every balance of this round was exact: out is the final state
+        if chains is None:
+            chains = {}
+            for k, s in enumerate(sender.tolist()):
+                chains.setdefault(s, []).append(k)
+        got_of = dict(zip(undecided.tolist(), got.tolist()))
+        for chain in chains.values():
+            for k in chain:
+                if verdicts[k] != -1:
+                    continue
+                verdicts[k] = got_of[k]
+                if got_of[k] != 1:
+                    break
+    verdicts = [int(v) for v in verdicts]
+    return verdicts, out[3:], out[1], rounds
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96
