@@ -11,12 +11,13 @@ import pytest
 
 from oracle import coracle as co
 from oracle import pyref as pr
+from tests import msm_reach as mr
 from zero_chain_b200 import groth16 as zk
 from zero_chain_b200 import synthetic as sy
 
 pytestmark = pytest.mark.gpu
 
-CHUNK = 4096              # entries per chunk of the coarse scatter, and the least tile length
+CHUNK = mr.COARSE_CHUNK   # entries per chunk of the coarse scatter, and the least tile length (checked against msm.cuh)
 
 
 @pytest.fixture(scope="module")
