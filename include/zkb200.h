@@ -341,6 +341,43 @@ int zk_balances_confidential_block_device(zk_ctx *ctx, size_t n_accounts, const 
                                           const uint32_t *d_recipient, const uint8_t *d_tx_points, const uint8_t *d_applied,
                                           uint8_t *d_balance_sender, uint8_t *d_balance_after, uint8_t *d_tx_status,
                                           uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags);
+/* ---- anonymous-transfer state updates of one block (what modules/anonymous-balances runs around each proof) ------------
+ * anonymous_transfer (modules/anonymous-balances/src/lib.rs:23-82, 169-232) for n_tx transactions over the module's own
+ * account table (AnonymousBalances storage, not EncryptedBalances).  ZK_ANON_RING = 12 members per transaction
+ * (core/proofs/src/constants.rs:1; the only ring the shipped anony_vk.dat accepts).  Each transaction rolls over its 12
+ * members (at an account's first touch, when due, as zk_balances_confidential_block does; the rollover stands whatever
+ * the verdict), then verify_anonymous_proof reads the 12 members' balances, and an applied transaction adds
+ * from_left_right(left_i, right_ciphertext) to member i's pending transfer.  A member listed twice is rolled over once and
+ * receives both additions.
+ * keys: n_accounts * 32 B, each account's EncKey: copied into the verifier inputs, never decoded here.
+ * balances / pendings / acct_flags: as zk_balances_confidential_block (bits 0-2: balance, pending, rollover due).
+ * members: n_tx * 12 account indices; tx_points: n_tx * 13 * 32 B = left_ciphertexts[0..12) | right_ciphertext;
+ * tx_extra: n_tx * 64 B = rvk | nonce; g_epoch: 32 B (LastGEpoch, one value per block).
+ * applied: n_tx bytes; transaction k is applied iff applied[k] == 1, so the verdicts of
+ *   zk_groth16_verify_points_batch(_device) can be passed unchanged (0, 2, 3 and 4 are all "not applied").
+ * enc_balances[k]: 12 * 64 B, the acc[] that verify_anonymous_proof reads (Ciphertext::zero() when absent).
+ * verify_points[k]: 52 * 32 B in verify_anonymous_proof's push order (12 keys, 12 left ciphertexts, the 12 acc left
+ *   points, the 12 acc right points, right_ciphertext, rvk, g_epoch, nonce), ready for zk_groth16_verify_points_batch with
+ *   n_points = 52.  What the verifier reads does not depend on applied.
+ * tx_status[k]: 0 applied; 1 not applied (applied[k] != 1); 2 a left / right point fails Point::read + as_prime_order (not
+ *   applied); 3 a member index >= n_accounts (the transaction touches nothing; its enc_balances and verify_points rows are
+ *   zero).  3 comes before 2 and 2 before 1.
+ * new_balances / new_pendings / new_flags: as zk_balances_confidential_block.
+ * ZK_ERR_DECODE when a touched account's stored ciphertext fails Ciphertext::read; zk_last_error names the lowest such
+ *   account, and the outputs are undefined.  ZK_ERR_INVALID for a NULL ctx, for a NULL account array when n_accounts > 0
+ *   or transaction array (g_epoch included) when n_tx > 0, for n_accounts above 2^22 and for n_tx above 2^18. */
+#define ZK_ANON_RING 12
+int zk_balances_anonymous_block(zk_ctx *ctx, size_t n_accounts, const uint8_t *keys, const uint8_t *balances, const uint8_t *pendings,
+                                const uint8_t *acct_flags, size_t n_tx, const uint32_t *members, const uint8_t *tx_points,
+                                const uint8_t *tx_extra, const uint8_t *g_epoch, const uint8_t *applied, uint8_t *enc_balances,
+                                uint8_t *verify_points, uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags);
+/* the same with device pointers (d_members 4-byte aligned); asynchronous on the context's stream.  A touched account that
+ * fails to decode is reported by the next zk_ctx_sync as ZK_ERR_DECODE, with the account named in zk_last_error */
+int zk_balances_anonymous_block_device(zk_ctx *ctx, size_t n_accounts, const uint8_t *d_keys, const uint8_t *d_balances,
+                                       const uint8_t *d_pendings, const uint8_t *d_acct_flags, size_t n_tx, const uint32_t *d_members,
+                                       const uint8_t *d_tx_points, const uint8_t *d_tx_extra, const uint8_t *d_g_epoch,
+                                       const uint8_t *d_applied, uint8_t *d_enc_balances, uint8_t *d_verify_points, uint8_t *d_tx_status,
+                                       uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

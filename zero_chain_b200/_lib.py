@@ -79,6 +79,8 @@ SIGNATURES = {
     "zk_elgamal_decrypt_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_balances_confidential_block": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_confidential_block_device": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "zk_balances_anonymous_block": (i32, [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "zk_balances_anonymous_block_device": (i32, [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),
 }
 

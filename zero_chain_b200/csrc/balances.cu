@@ -1,7 +1,8 @@
 // Confidential-transfer balance updates of one block on the device (balances.cuh): zk_balances_confidential_block and its
 // _device form.  One pass per stage, each one balances.cuh function per item and thread, all on the context's stream; the
 // workspace stays in the context.  The _device form only enqueues: a touched account that fails to read is left in an
-// error word of the context, which the host form (and zk_ctx_sync after the _device form) reads back.
+// error word of the context, which the host form (and zk_ctx_sync after the _device form) reads back.  The radix sort and
+// the segmented scan (zk_bal_sort, zk_bal_scan) also serve the anonymous-transfer block of anon_balances.cu.
 //
 // Like elgamal.cu, the translation unit holds only Fr arithmetic and is compiled with everything inlined (ZK_HOT).
 #define ZK_HOT 1
@@ -128,17 +129,6 @@ static __global__ void __launch_bounds__(BT) k_bal_finish_acct(size_t n_acct, si
     BAL_FOR(a, n_acct) bal_finish_acct(a, n_tx, touched, balances, pendings, flags, present, enc, new_balances, new_pendings, new_flags);
 }
 
-// carves the workspace out of one grow-only buffer, 256-byte aligned pieces
-struct Carve {
-    uint8_t *base = nullptr;
-    size_t off = 0;
-    template <class T> T *take(size_t count) {
-        T *p = reinterpret_cast<T *>(base ? base + off : nullptr);
-        off += (count * sizeof(T) + 255) & ~(size_t)255;
-        return p;
-    }
-};
-
 struct BalWork {
     uint32_t *keys0, *keys1, *vals0, *vals1, *hist, *totals;
     uint8_t *touched, *recv_any, *rflags, *present, *ok, *has, *head;
@@ -183,6 +173,55 @@ static int key_passes(size_t n_acct) {
     return bits <= BAL_RADIX_BITS ? 1 : (bits + BAL_RADIX_BITS - 1) / BAL_RADIX_BITS;
 }
 
+int zk_bal_sort(zk_ctx *ctx, size_t ne, size_t n_acct, uint32_t *keys0, uint32_t *keys1, uint32_t *vals0, uint32_t *vals1, uint32_t *hist,
+                uint32_t *totals, const uint32_t **keys, const uint32_t **vals) {
+    // stable sort of the elements by key.  (The MSM's counting sorts in msm.cuh scatter with atomicAdd cursors, so the
+    // order inside a bucket is not kept; here the order inside an account is the transaction order the scan needs.)
+    // One thread walks BAL_SORT_TILE consecutive elements in order, counting and then placing them through its own
+    // column of the [digit][tile] counters in global memory.
+    cudaStream_t st = ctx->stream;
+    const size_t n_tiles = (ne + BAL_SORT_TILE - 1) / BAL_SORT_TILE;
+    const int passes = key_passes(n_acct);
+    const size_t n_cnt = BAL_RADIX * n_tiles;
+    size_t segs = (n_cnt + SCAN_MIN_SEG - 1) / SCAN_MIN_SEG;
+    segs = segs < SCAN_SEGMENTS ? segs : SCAN_SEGMENTS;
+    const size_t seg = (n_cnt + segs - 1) / segs;
+    uint32_t *kin = keys0, *vin = nullptr, *kout = keys1, *vout = vals1;
+    for (int p = 0; p < passes; p++) {
+        ZK_CUDA(cudaMemsetAsync(hist, 0, sizeof(uint32_t) * BAL_RADIX * n_tiles, st));
+        k_bal_radix_hist<<<grid(ctx, n_tiles), BT, 0, st>>>(ne, kin, BAL_RADIX_BITS * p, n_tiles, hist);
+        if (segs > 1) {
+            k_bal_counter_sums<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(hist, n_cnt, seg, totals);
+            k_bal_counter_scan<<<1, SCAN_THREADS, 0, st>>>(totals, segs, segs, nullptr);
+        }
+        k_bal_counter_scan<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(hist, n_cnt, seg, segs > 1 ? totals : nullptr);
+        k_bal_radix_scatter<<<grid(ctx, n_tiles), BT, 0, st>>>(ne, kin, vin, BAL_RADIX_BITS * p, n_tiles, hist, kout, vout);
+        kin = kout; vin = vout;
+        kout = kin == keys1 ? keys0 : keys1;
+        vout = vin == vals1 ? vals0 : vals1;
+    }
+    *keys = kin;
+    *vals = vin;
+    ZK_CUDA(cudaGetLastError());
+    return ZK_OK;
+}
+
+int zk_bal_scan(zk_ctx *ctx, const uint32_t *keys, const uint32_t *vals, const Pair *delta, size_t L, const size_t *lvl_n,
+                Pair *const *lvl_agg, Pair *const *lvl_out, uint8_t *const *lvl_head) {
+    // segmented exclusive scan: up the levels, then down
+    cudaStream_t st = ctx->stream;
+    const size_t ne = lvl_n[0];
+    k_bal_heads<<<grid(ctx, ne), BT, 0, st>>>(ne, keys, lvl_head[0]);
+    for (size_t l = 0; l + 1 < L; l++)
+        k_bal_scan_up<<<grid(ctx, lvl_n[l + 1]), BT, 0, st>>>(lvl_n[l], l ? lvl_agg[l] : delta, l ? nullptr : vals, lvl_head[l],
+                                                              lvl_agg[l + 1], lvl_head[l + 1]);
+    for (size_t l = L; l-- > 0;)
+        k_bal_scan_down<<<grid(ctx, (lvl_n[l] + BAL_SCAN_CHUNK - 1) / BAL_SCAN_CHUNK), BT, 0, st>>>(
+            lvl_n[l], l ? lvl_agg[l] : delta, l ? nullptr : vals, lvl_head[l], l + 1 < L ? lvl_out[l + 1] : nullptr, l == 0, lvl_out[l]);
+    ZK_CUDA(cudaGetLastError());
+    return ZK_OK;
+}
+
 static int run_block(zk_ctx *ctx, size_t n_acct, const uint8_t *balances, const uint8_t *pendings, const uint8_t *acct_flags, size_t n_tx,
                      const uint32_t *sender, const uint32_t *recipient, const uint8_t *tx_points, const uint8_t *applied,
                      uint8_t *balance_sender, uint8_t *balance_after, uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings,
@@ -194,7 +233,7 @@ static int run_block(zk_ctx *ctx, size_t n_acct, const uint8_t *balances, const 
     Carve c;
     c.base = buf.as<uint8_t>();
     carve(c, w, n_tx, n_acct);
-    const size_t ne = 2 * n_tx, np = 4 * n_tx + 4 * n_acct, n_tiles = (ne + BAL_SORT_TILE - 1) / BAL_SORT_TILE;
+    const size_t ne = 2 * n_tx, np = 4 * n_tx + 4 * n_acct;
     const uint32_t na = (uint32_t)n_acct;
 
     ZK_CUDA(cudaMemsetAsync(w.touched, 0, 2 * n_acct, st));
@@ -207,40 +246,9 @@ static int run_block(zk_ctx *ctx, size_t n_acct, const uint8_t *balances, const 
     k_bal_account<<<grid(ctx, n_acct), BT, 0, st>>>(n_acct, n_tx, acct_flags, w.touched, w.dec, w.ok, w.roll_b, w.roll_p, w.rflags, bad);
     ZK_CUDA(cudaGetLastError());
     if (n_tx) {
-        // stable sort of the elements by key.  (The MSM's counting sorts in msm.cuh scatter with atomicAdd cursors, so the
-        // order inside a bucket is not kept; here the order inside an account is the transaction order the scan needs.)
-        // One thread walks BAL_SORT_TILE consecutive elements in order, counting and then placing them through its own
-        // column of the [digit][tile] counters in global memory.
-        const int passes = key_passes(n_acct);
-        const size_t n_cnt = BAL_RADIX * n_tiles;
-        size_t segs = (n_cnt + SCAN_MIN_SEG - 1) / SCAN_MIN_SEG;
-        segs = segs < SCAN_SEGMENTS ? segs : SCAN_SEGMENTS;
-        const size_t seg = (n_cnt + segs - 1) / segs;
-        uint32_t *kin = w.keys0, *vin = nullptr, *kout = w.keys1, *vout = w.vals1;
-        for (int p = 0; p < passes; p++) {
-            ZK_CUDA(cudaMemsetAsync(w.hist, 0, sizeof(uint32_t) * BAL_RADIX * n_tiles, st));
-            k_bal_radix_hist<<<grid(ctx, n_tiles), BT, 0, st>>>(ne, kin, BAL_RADIX_BITS * p, n_tiles, w.hist);
-            if (segs > 1) {
-                k_bal_counter_sums<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(w.hist, n_cnt, seg, w.totals);
-                k_bal_counter_scan<<<1, SCAN_THREADS, 0, st>>>(w.totals, segs, segs, nullptr);
-            }
-            k_bal_counter_scan<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(w.hist, n_cnt, seg, segs > 1 ? w.totals : nullptr);
-            k_bal_radix_scatter<<<grid(ctx, n_tiles), BT, 0, st>>>(ne, kin, vin, BAL_RADIX_BITS * p, n_tiles, w.hist, kout, vout);
-            kin = kout; vin = vout;
-            kout = kin == w.keys1 ? w.keys0 : w.keys1;
-            vout = vin == w.vals1 ? w.vals0 : w.vals1;
-        }
-        const uint32_t *keys = kin, *vals = vin;
-        // segmented exclusive scan: up the levels, then down
-        k_bal_heads<<<grid(ctx, ne), BT, 0, st>>>(ne, keys, w.head);
-        const size_t L = w.lvl_n.size();
-        for (size_t l = 0; l + 1 < L; l++)
-            k_bal_scan_up<<<grid(ctx, w.lvl_n[l + 1]), BT, 0, st>>>(w.lvl_n[l], l ? w.lvl_agg[l] : w.delta, l ? nullptr : vals,
-                                                                    w.lvl_head[l], w.lvl_agg[l + 1], w.lvl_head[l + 1]);
-        for (size_t l = L; l-- > 0;)
-            k_bal_scan_down<<<grid(ctx, (w.lvl_n[l] + BAL_SCAN_CHUNK - 1) / BAL_SCAN_CHUNK), BT, 0, st>>>(
-                w.lvl_n[l], l ? w.lvl_agg[l] : w.delta, l ? nullptr : vals, w.lvl_head[l], l + 1 < L ? w.lvl_out[l + 1] : nullptr,
-                l == 0, w.lvl_out[l]);
+        const uint32_t *keys, *vals;
+        ZK_TRY(zk_bal_sort(ctx, ne, n_acct, w.keys0, w.keys1, w.vals0, w.vals1, w.hist, w.totals, &keys, &vals));
+        ZK_TRY(zk_bal_scan(ctx, keys, vals, w.delta, w.lvl_n.size(), w.lvl_n.data(), w.lvl_agg.data(), w.lvl_out.data(), w.lvl_head.data()));
         k_bal_tx_points<<<grid(ctx, ne), BT, 0, st>>>(ne, na, keys, vals, w.excl, w.delta, w.roll_b, w.rflags, tx_status, w.pts, w.tot, w.has);
         ZK_CUDA(cudaGetLastError());
     }

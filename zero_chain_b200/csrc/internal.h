@@ -38,6 +38,17 @@ struct DevBuf {
     template <class T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
+// carves a workspace out of one grow-only buffer, 256-byte aligned pieces (base NULL: only sums the size)
+struct Carve {
+    uint8_t *base = nullptr;
+    size_t off = 0;
+    template <class T> T *take(size_t count) {
+        T *p = reinterpret_cast<T *>(base ? base + off : nullptr);
+        off += (count * sizeof(T) + 255) & ~(size_t)255;
+        return p;
+    }
+};
+
 // one cached set of NTT twiddle tables (ntt.cu)
 struct NttSlot { unsigned log_n = 0; bool valid = false; uint64_t last_use = 0; DevBuf w, g, gi, consts; };
 
@@ -74,7 +85,8 @@ struct zk_ctx {
     // zk_elgamal_decrypt_batch (elgamal.cu): the encodings of i P_G for i < 10^6 and their index, built by the first call
     DevBuf eg_table, eg_index;
     bool eg_ready = false;
-    DevBuf bal, bal_io;            // zk_balances_confidential_block (balances.cu): workspace, and the host form's staging
+    DevBuf bal, bal_io;            // zk_balances_confidential_block (balances.cu) and zk_balances_anonymous_block
+                                   // (anon_balances.cu): workspace, and the host forms' staging
     DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;
@@ -120,8 +132,19 @@ int zk_fr_quotient(zk_ctx *ctx, const void *d_abc, unsigned log_m, size_t batch,
 int zk_fr_into_repr(zk_ctx *ctx, const void *d_h, unsigned log_m, size_t n_out, size_t n_total, size_t batch, void *d_scal);
 int zk_fr_blinding_terms(zk_ctx *ctx, const void *d_r, const void *d_s, size_t batch, void *d_out);
 int zk_check_err_flag(zk_ctx *ctx);
-// d_err[ZK_ERR_SLOT_ACCOUNT]: ~(the lowest account whose stored ciphertext failed to read) in zk_balances_confidential_block, 0: none
+// d_err[ZK_ERR_SLOT_ACCOUNT]: ~(the lowest account whose stored ciphertext failed to read) in zk_balances_confidential_block
+// and zk_balances_anonymous_block, 0: none
 constexpr int ZK_ERR_SLOT_ACCOUNT = 2;
+// balances.cu's passes over a block's elements, shared with anon_balances.cu, enqueued on ctx->stream:
+//   zk_bal_sort  stable LSD radix sort of ne keys (each <= 2 n_acct; keys0 holds them, keys1 / vals0 / vals1 / hist /
+//                totals are workspace of balances.cuh's sizes) with the element ids; *keys / *vals: the sorted pair
+//   zk_bal_scan  segmented exclusive scan of delta[vals[j]] in key order over L levels (lvl_n[0] = ne; level l >= 1 has
+//                lvl_n[l] items and its lvl_agg / lvl_out / lvl_head; lvl_out[0] receives the scan, lvl_head[0] the heads)
+namespace zkbal { struct Pair; }
+int zk_bal_sort(zk_ctx *ctx, size_t ne, size_t n_acct, uint32_t *keys0, uint32_t *keys1, uint32_t *vals0, uint32_t *vals1, uint32_t *hist,
+                uint32_t *totals, const uint32_t **keys, const uint32_t **vals);
+int zk_bal_scan(zk_ctx *ctx, const uint32_t *keys, const uint32_t *vals, const zkbal::Pair *delta, size_t L, const size_t *lvl_n,
+                zkbal::Pair *const *lvl_agg, zkbal::Pair *const *lvl_out, uint8_t *const *lvl_head);
 // lane-parallel verifier kernels (pairing_lanes.cu)
 void zk_launch_miller_lanes(cudaStream_t st, size_t n, const void *a, const void *acc, const void *c, const void *coef_b, const void *gamma, int gamma_inf,
                             const void *delta, int delta_inf, const uint8_t *status, void *f);

@@ -664,6 +664,121 @@ def import_confidential_block(ctx: Context, pvk: PreparedVerifyingKey, accounts,
     return verdicts, out[3:], out[1], rounds
 
 
+# ---- anonymous-transfer state updates of one block (modules/anonymous-balances/src/lib.rs:23-82, 169-232) ---------------
+# statuses as BLOCK_*; account flags as ACCOUNT_*
+
+
+def anonymous_block(ctx: Context, keys, balances, pendings, flags, members, tx_points, tx_extra, g_epoch, applied):
+    """rollover of the 12 ring members, the balances verify_anonymous_proof reads, and add_pending_transfer for every member
+    of the applied transactions (zk_balances_anonymous_block).  keys: 32 bytes per account (its EncKey); balances /
+    pendings / flags: as confidential_block; members: ANONIMITY_SIZE account indices per transaction (flat or one row per
+    transaction); tx_points: 416 bytes per transaction (left_ciphertexts | right_ciphertext); tx_extra: 64 bytes per
+    transaction (rvk | nonce); g_epoch: 32 bytes; applied: one byte per transaction, applied when 1 (a verdict of
+    verify_proofs_with_points passes unchanged).  Returns (enc_balances, verify_points, status, new_balances, new_pendings,
+    new_flags) as bytes: 768 and 1664 bytes per transaction for the first two.  Raises SynthesisError(ZK_ERR_DECODE) naming
+    the account when a touched account's stored ciphertext does not read."""
+    n_acct = len(flags)
+    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1).astype(np.uint32))
+    assert len(mem) % ANONIMITY_SIZE == 0
+    n_tx = len(mem) // ANONIMITY_SIZE
+    ky, bal, pend, fl = _cat(keys, 32), _cat(balances, 64), _cat(pendings, 64), bytes(flags)
+    tp, tx, ge, ap = _cat(tx_points, 32 * (ANONIMITY_SIZE + 1)), _cat(tx_extra, 64), _pt32(g_epoch), bytes(applied)
+    assert len(ky) == 32 * n_acct and len(bal) == len(pend) == 64 * n_acct
+    assert len(tp) == 32 * (ANONIMITY_SIZE + 1) * n_tx and len(tx) == 64 * n_tx and len(ap) == n_tx
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    eb = np.zeros(max(64 * ANONIMITY_SIZE * n_tx, 1), np.uint8)
+    vp = np.zeros(max(32 * ANONYMOUS_POINTS * n_tx, 1), np.uint8)
+    st = np.zeros(max(n_tx, 1), np.uint8)
+    nb, npd = np.zeros(max(64 * n_acct, 1), np.uint8), np.zeros(max(64 * n_acct, 1), np.uint8)
+    nf = np.zeros(max(n_acct, 1), np.uint8)
+    _ck(_lib.lib().zk_balances_anonymous_block(ctx._h, n_acct, _p(buf(ky)), _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n_tx,
+                                               _p(mem if n_tx else np.zeros(1, np.uint32)), _p(buf(tp)), _p(buf(tx)), _p(buf(ge)),
+                                               _p(buf(ap)), _p(eb), _p(vp), _p(st), _p(nb), _p(npd), _p(nf)))
+    return (eb[:64 * ANONIMITY_SIZE * n_tx].tobytes(), vp[:32 * ANONYMOUS_POINTS * n_tx].tobytes(), st[:n_tx].tobytes(),
+            nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes())
+
+
+def anonymous_block_device(ctx: Context, n_accounts: int, d_keys_ptr: int, d_balances_ptr: int, d_pendings_ptr: int, d_flags_ptr: int,
+                           n_tx: int, d_members_ptr: int, d_tx_points_ptr: int, d_tx_extra_ptr: int, d_g_epoch_ptr: int, d_applied_ptr: int,
+                           d_enc_balances_ptr: int, d_verify_points_ptr: int, d_status_ptr: int, d_new_balances_ptr: int,
+                           d_new_pendings_ptr: int, d_new_flags_ptr: int):
+    """The same on device pointers (d_members: uint32), asynchronous on the context's stream; ctx.sync() raises
+    SynthesisError(ZK_ERR_DECODE) naming a touched account whose stored ciphertext did not read."""
+    v = lambda x: C.c_void_p(x) if x else None
+    _ck(_lib.lib().zk_balances_anonymous_block_device(ctx._h, n_accounts, v(d_keys_ptr), v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr),
+                                                      n_tx, v(d_members_ptr), v(d_tx_points_ptr), v(d_tx_extra_ptr), v(d_g_epoch_ptr),
+                                                      v(d_applied_ptr), v(d_enc_balances_ptr), v(d_verify_points_ptr), v(d_status_ptr),
+                                                      v(d_new_balances_ptr), v(d_new_pendings_ptr), v(d_new_flags_ptr)))
+
+
+class AnonymousTx:
+    """One anonymous_transfer extrinsic (lib.rs:23-30) with its ring as indices into the block's account table: the 12
+    members (enc_keys), their left ciphertexts, right_ciphertext, the signer's rvk and the nonce."""
+
+    def __init__(self, members, left_ciphertexts, right_ciphertext, rvk, nonce):
+        self.members = [int(m) for m in members]
+        self.left_ciphertexts = [_pt32(c) for c in left_ciphertexts]
+        if len(self.members) != ANONIMITY_SIZE or len(self.left_ciphertexts) != ANONIMITY_SIZE:
+            raise ValueError("AnonymousTx: a ring of %d members and %d left ciphertexts; the anonymous key takes %d"
+                             % (len(self.members), len(self.left_ciphertexts), ANONIMITY_SIZE))
+        self.right_ciphertext, self.rvk, self.nonce = _pt32(right_ciphertext), _pt32(rvk), _pt32(nonce)
+
+    def points(self) -> bytes:
+        return b"".join(self.left_ciphertexts) + self.right_ciphertext
+
+
+def import_anonymous_block(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
+    """Verify and apply a block of anonymous transfers the way the runtime does, with the state, the verifier's inputs and
+    the verdicts on the device.  accounts = (keys, balances, pendings, flags) as anonymous_block takes them; txs:
+    AnonymousTx list; g_epoch: the block's 32-byte LastGEpoch; proofs: 192 bytes each.
+
+    A transfer changes pending balances only, so what each proof is checked against (its members' balances after their
+    rollover) does not depend on any verdict.  One upload, then: anonymous_block_device with nothing applied gives every
+    transaction's 52 public-input points; verify_proofs_with_points_device checks the proofs on them; anonymous_block_device
+    again, with the verdict buffer as the mask, gives the final state; one download.
+
+    Returns (verdicts, (new_balances, new_pendings, new_flags), enc_balances): the reference's verdict per transaction (1
+    passes; the other values as verify_proofs_with_points) and the 12 balances (768 bytes) each transaction's proof was
+    checked against.  Raises ValueError for an account index out of range, SynthesisError(ZK_ERR_DECODE) for a touched
+    account whose stored ciphertext does not read."""
+    import torch
+    keys, balances, pendings, flags = accounts
+    n_acct, n = len(flags), len(txs)
+    if any(not all(0 <= m < n_acct for m in t.members) for t in txs):
+        raise ValueError("import_anonymous_block: account index out of range")
+    proofs = _cat(proofs, 192)
+    assert len(proofs) == 192 * n
+    ky, bal, pend, fl, ge = _cat(keys, 32), _cat(balances, 64), _cat(pendings, 64), bytes(flags), _pt32(g_epoch)
+    assert len(ky) == 32 * n_acct and len(bal) == len(pend) == 64 * n_acct
+    if not n:
+        return [], (bal, pend, fl), b""
+    members = np.array([t.members for t in txs], np.uint32).reshape(-1)
+    # one host buffer of the inputs (members first, 4-byte aligned), one of the outputs; each one transfer
+    parts = [members.tobytes(), ky, bal, pend, fl, b"".join(t.points() for t in txs), b"".join(t.rvk + t.nonce for t in txs), ge, proofs]
+    offs = np.cumsum([0] + [len(p) for p in parts]).tolist()
+    dev = torch.device("cuda", ctx.device)
+    d_in = torch.frombuffer(bytearray(b"".join(parts)), dtype=torch.uint8).to(dev)
+    sizes = [64 * ANONIMITY_SIZE * n, 32 * ANONYMOUS_POINTS * n, n, 64 * n_acct, 64 * n_acct, n_acct, n, n]
+    oo = np.cumsum([0] + sizes).tolist()
+    d_out = torch.zeros(oo[-1], dtype=torch.uint8, device=dev)     # the last n bytes: the all-zero mask of the first call
+    torch.cuda.current_stream(dev).synchronize()                    # the context's stream is not torch's
+    pi = lambda i: d_in.data_ptr() + offs[i]
+    po = lambda i: d_out.data_ptr() + oo[i]
+    state = lambda applied: anonymous_block_device(ctx, n_acct, pi(1), pi(2), pi(3), pi(4), n, pi(0), pi(5), pi(6), pi(7), applied,
+                                                   po(0), po(1), po(2), po(3), po(4), po(5))
+    state(po(7))
+    if pvk.ctx is not ctx:
+        ctx.sync()
+    verify_proofs_with_points_device(pvk, n, pi(8), po(1), ANONYMOUS_POINTS, po(6))
+    if pvk.ctx is not ctx:
+        pvk.ctx.sync()
+    state(po(6))
+    ctx.sync()
+    host = d_out[:oo[7]].cpu().numpy().tobytes()
+    verdicts = [int(v) for v in host[oo[6]:oo[7]]]
+    return verdicts, (host[oo[3]:oo[4]], host[oo[4]:oo[5]], host[oo[5]:oo[6]]), host[oo[0]:oo[1]]
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96
