@@ -61,8 +61,13 @@ struct XYZZ {
     }
     ZK_DEV XYZZ neg() const { XYZZ r = *this; r.y = y.neg(); return r; }
 
+    // The doubling formulas, always inlined.  add() and add_mixed() use these in their equal-points branch instead of calling
+    // dbl() / dbl_affine(): where those are separate functions (the units that are not ZK_HOT) the callee reloads uniform
+    // registers, and a call made by some lanes of a diverged warp overwrote the uniform memory descriptor that the other
+    // lanes' loads in add() still used (k_ic_sum: "an illegal instruction was encountered" when one proof of a warp hit the
+    // doubling branch).  Inlined, the whole branch is in one function and the register allocation sees every use.
     // 2 * (affine p)   (mdbl-2008-s-1)
-    ZK_PTFN static XYZZ dbl_affine(const Affine<F> &p) {
+    ZK_DEV static XYZZ dbl_affine_inl(const Affine<F> &p) {
         if (p.is_inf()) return inf();
         F u = p.y.dbl(), v = u.sqr(), w = u * v, s = p.x * v;
         F xx = p.x.sqr(), m = xx.dbl() + xx;
@@ -73,7 +78,7 @@ struct XYZZ {
         return r;
     }
     // 2 * this   (dbl-2008-s-1)
-    ZK_PTFN XYZZ dbl() const {
+    ZK_DEV XYZZ dbl_inl() const {
         if (is_inf()) return *this;
         F u = y.dbl(), v = u.sqr(), w = u * v, s = x * v;
         F xx = x.sqr(), m = xx.dbl() + xx;
@@ -83,6 +88,8 @@ struct XYZZ {
         r.zz = v * zz; r.zzz = w * zzz;
         return r;
     }
+    ZK_PTFN static XYZZ dbl_affine(const Affine<F> &p) { return dbl_affine_inl(p); }
+    ZK_PTFN XYZZ dbl() const { return dbl_inl(); }
     // this += affine p   (madd-2008-s), p optionally negated by the caller beforehand
     ZK_PTFN void add_mixed(const Affine<F> &p) {
         if (p.is_inf()) return;
@@ -90,7 +97,7 @@ struct XYZZ {
         F u2 = p.x * zz, s2 = p.y * zzz;
         F pp_ = u2 - x, r = s2 - y;
         if (pp_.is_zero()) {
-            if (r.is_zero()) *this = dbl_affine(p); else *this = inf();
+            if (r.is_zero()) *this = dbl_affine_inl(p); else *this = inf();
             return;
         }
         F pp = pp_.sqr(), ppp = pp_ * pp, q = x * pp;
@@ -106,7 +113,7 @@ struct XYZZ {
         F u1 = x * o.zz, u2 = o.x * zz, s1 = y * o.zzz, s2 = o.y * zzz;
         F pp_ = u2 - u1, r = s2 - s1;
         if (pp_.is_zero()) {
-            if (r.is_zero()) *this = dbl(); else *this = inf();
+            if (r.is_zero()) *this = dbl_inl(); else *this = inf();
             return;
         }
         F pp = pp_.sqr(), ppp = pp_ * pp, q = u1 * pp;
