@@ -378,6 +378,53 @@ int zk_balances_anonymous_block_device(zk_ctx *ctx, size_t n_accounts, const uin
                                        const uint8_t *d_tx_points, const uint8_t *d_tx_extra, const uint8_t *d_g_epoch,
                                        const uint8_t *d_applied, uint8_t *d_enc_balances, uint8_t *d_verify_points, uint8_t *d_tx_status,
                                        uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags);
+/* ---- encrypted-asset calls of one block (what modules/encrypted-assets runs around each proof) --------------------------
+ * confidential_transfer, issue and destroy (modules/encrypted-assets/src/lib.rs:32-215, 266-358) for n_tx transactions, in
+ * order, over a table of n_slots slots: one slot per (AssetId, EncKey), numbered by the caller.
+ * balances / pendings: n_slots * 64 B; slot_flags[s]: bit 0 balance present, bit 1 pending present, bit 2 rollover due
+ *   (LastRollOver, or 0 when absent, < current_epoch, worked out by the caller); bits 3-7 are kept.
+ * kind[k]: 0 confidential_transfer, 1 issue, 2 destroy.
+ * slot_a[k]: the sender's slot, the issuer's (new asset id, issuer) slot, or the owner's slot; slot_b[k]: the recipient's
+ *   slot, read for transfers only.  Asset ids come from the caller, who knows the issue verdicts before choosing the
+ *   issuer's slot; nothing here numbers assets.
+ * tx_points: n_tx * 128 B.  Transfer: amount_sender | amount_recipient | fee_sender | randomness; issue: total | ignored |
+ *   ignored | randomness; destroy: ignored.
+ * applied[k]: transaction k is applied iff applied[k] == 1, so verifier verdicts pass unchanged.
+ * A transfer rolls over its sender, then its recipient, at a due slot's first transfer touch (balance = (balance or zero) +
+ *   (pending or zero), present; pending absent; the rollover stands whatever the verdict), then, when applied, balance(a)
+ *   -= (amount_sender + fee_sender, 2 randomness), an absent balance staying absent, and pending(b) += (amount_recipient,
+ *   randomness).  An applied issue sets balance(a) = (total, randomness) (TotalSupply holds the same ciphertext); an applied
+ *   destroy takes balance(a) and pending(a), both absent after.  Neither rolls over, and neither clears the due bit.
+ * balance_sender[k]: 64 B.  A transfer: the sender's balance verify_confidential_proof reads (Ciphertext::zero() when
+ *   absent); 64 zero bytes for the other kinds.
+ * balance_after[k]: 64 B, the sender's balance after an applied transfer (the event); other entries are left as they are.
+ * event_ct[k] / event_flags[k]: 128 B / 1 B, written for applied issues and destroys only.  An issue: its total ciphertext
+ *   | 64 zero bytes, flags 1.  A destroy: the taken balance | the taken pending, an absent one as 64 zero bytes; flags bit 0
+ *   / bit 1 tell which were present.
+ * tx_status[k]: 0 applied; 1 not applied (applied[k] != 1); 2 a point the call reads fails Point::read + as_prime_order (a
+ *   transfer's four, an issue's total and randomness; not applied, and a transfer's rollovers still stand); 3 a slot index
+ *   >= n_slots or an unknown kind (the transaction touches nothing).  3 comes before 2 and 2 before 1.
+ * new_balances / new_pendings / new_flags: the state after the block.  A slot no valid transaction names is copied through
+ *   byte for byte; a named slot's absent ciphertexts are 64 zero bytes, its flags keep bits 3-7, and bit 2 is cleared only
+ *   when a transfer touched it.
+ * Every ciphertext written is a Point::write encoding.  Where the module moves stored bytes unchanged (a rollover into an
+ *   absent balance, destroy's take), this differs only for an identity point stored with the x-sign bit set, which
+ *   Point::read accepts.
+ * ZK_ERR_DECODE when a named slot's stored ciphertext (balance or pending, when present) fails Ciphertext::read;
+ *   zk_last_error names the lowest such slot, and the outputs are undefined.  ZK_ERR_INVALID for a NULL ctx, for a NULL
+ *   slot array when n_slots > 0 or transaction array when n_tx > 0, for n_slots above 2^22 and for n_tx above 2^20 (6 sort
+ *   elements per transaction).  n_tx = 0 gives the state back unchanged. */
+int zk_assets_block(zk_ctx *ctx, size_t n_slots, const uint8_t *balances, const uint8_t *pendings, const uint8_t *slot_flags,
+                    size_t n_tx, const uint8_t *kind, const uint32_t *slot_a, const uint32_t *slot_b, const uint8_t *tx_points,
+                    const uint8_t *applied, uint8_t *balance_sender, uint8_t *balance_after, uint8_t *event_ct, uint8_t *event_flags,
+                    uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags);
+/* the same with device pointers (d_slot_a / d_slot_b 4-byte aligned); asynchronous on the context's stream.  A named slot
+ * that fails to decode is reported by the next zk_ctx_sync as ZK_ERR_DECODE, with the slot named in zk_last_error */
+int zk_assets_block_device(zk_ctx *ctx, size_t n_slots, const uint8_t *d_balances, const uint8_t *d_pendings, const uint8_t *d_slot_flags,
+                           size_t n_tx, const uint8_t *d_kind, const uint32_t *d_slot_a, const uint32_t *d_slot_b, const uint8_t *d_tx_points,
+                           const uint8_t *d_applied, uint8_t *d_balance_sender, uint8_t *d_balance_after, uint8_t *d_event_ct,
+                           uint8_t *d_event_flags, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
+                           uint8_t *d_new_flags);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

@@ -173,6 +173,21 @@ static int key_passes(size_t n_acct) {
     return bits <= BAL_RADIX_BITS ? 1 : (bits + BAL_RADIX_BITS - 1) / BAL_RADIX_BITS;
 }
 
+int zk_bal_prefix_sum(zk_ctx *ctx, uint32_t *c, size_t n, uint32_t *totals) {
+    // up to SCAN_SEGMENTS segments of at least SCAN_MIN_SEG counters: their sums, a scan of the sums, each segment's scan
+    cudaStream_t st = ctx->stream;
+    size_t segs = (n + SCAN_MIN_SEG - 1) / SCAN_MIN_SEG;
+    segs = segs < SCAN_SEGMENTS ? segs : SCAN_SEGMENTS;
+    const size_t seg = (n + segs - 1) / segs;
+    if (segs > 1) {
+        k_bal_counter_sums<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(c, n, seg, totals);
+        k_bal_counter_scan<<<1, SCAN_THREADS, 0, st>>>(totals, segs, segs, nullptr);
+    }
+    k_bal_counter_scan<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(c, n, seg, segs > 1 ? totals : nullptr);
+    ZK_CUDA(cudaGetLastError());
+    return ZK_OK;
+}
+
 int zk_bal_sort(zk_ctx *ctx, size_t ne, size_t n_acct, uint32_t *keys0, uint32_t *keys1, uint32_t *vals0, uint32_t *vals1, uint32_t *hist,
                 uint32_t *totals, const uint32_t **keys, const uint32_t **vals) {
     // stable sort of the elements by key.  (The MSM's counting sorts in msm.cuh scatter with atomicAdd cursors, so the
@@ -182,19 +197,11 @@ int zk_bal_sort(zk_ctx *ctx, size_t ne, size_t n_acct, uint32_t *keys0, uint32_t
     cudaStream_t st = ctx->stream;
     const size_t n_tiles = (ne + BAL_SORT_TILE - 1) / BAL_SORT_TILE;
     const int passes = key_passes(n_acct);
-    const size_t n_cnt = BAL_RADIX * n_tiles;
-    size_t segs = (n_cnt + SCAN_MIN_SEG - 1) / SCAN_MIN_SEG;
-    segs = segs < SCAN_SEGMENTS ? segs : SCAN_SEGMENTS;
-    const size_t seg = (n_cnt + segs - 1) / segs;
     uint32_t *kin = keys0, *vin = nullptr, *kout = keys1, *vout = vals1;
     for (int p = 0; p < passes; p++) {
         ZK_CUDA(cudaMemsetAsync(hist, 0, sizeof(uint32_t) * BAL_RADIX * n_tiles, st));
         k_bal_radix_hist<<<grid(ctx, n_tiles), BT, 0, st>>>(ne, kin, BAL_RADIX_BITS * p, n_tiles, hist);
-        if (segs > 1) {
-            k_bal_counter_sums<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(hist, n_cnt, seg, totals);
-            k_bal_counter_scan<<<1, SCAN_THREADS, 0, st>>>(totals, segs, segs, nullptr);
-        }
-        k_bal_counter_scan<<<(unsigned)segs, SCAN_THREADS, 0, st>>>(hist, n_cnt, seg, segs > 1 ? totals : nullptr);
+        ZK_TRY(zk_bal_prefix_sum(ctx, hist, BAL_RADIX * n_tiles, totals));
         k_bal_radix_scatter<<<grid(ctx, n_tiles), BT, 0, st>>>(ne, kin, vin, BAL_RADIX_BITS * p, n_tiles, hist, kout, vout);
         kin = kout; vin = vout;
         kout = kin == keys1 ? keys0 : keys1;

@@ -85,8 +85,8 @@ struct zk_ctx {
     // zk_elgamal_decrypt_batch (elgamal.cu): the encodings of i P_G for i < 10^6 and their index, built by the first call
     DevBuf eg_table, eg_index;
     bool eg_ready = false;
-    DevBuf bal, bal_io;            // zk_balances_confidential_block (balances.cu) and zk_balances_anonymous_block
-                                   // (anon_balances.cu): workspace, and the host forms' staging
+    DevBuf bal, bal_io;            // zk_balances_confidential_block (balances.cu), zk_balances_anonymous_block
+                                   // (anon_balances.cu) and zk_assets_block (assets.cu): workspace, and the host forms' staging
     DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;
@@ -133,14 +133,17 @@ int zk_fr_into_repr(zk_ctx *ctx, const void *d_h, unsigned log_m, size_t n_out, 
 int zk_fr_blinding_terms(zk_ctx *ctx, const void *d_r, const void *d_s, size_t batch, void *d_out);
 int zk_check_err_flag(zk_ctx *ctx);
 // d_err[ZK_ERR_SLOT_ACCOUNT]: ~(the lowest account whose stored ciphertext failed to read) in zk_balances_confidential_block
-// and zk_balances_anonymous_block, 0: none
+// and zk_balances_anonymous_block (the lowest slot in zk_assets_block), 0: none
 constexpr int ZK_ERR_SLOT_ACCOUNT = 2;
 // balances.cu's passes over a block's elements, shared with anon_balances.cu, enqueued on ctx->stream:
 //   zk_bal_sort  stable LSD radix sort of ne keys (each <= 2 n_acct; keys0 holds them, keys1 / vals0 / vals1 / hist /
 //                totals are workspace of balances.cuh's sizes) with the element ids; *keys / *vals: the sorted pair
 //   zk_bal_scan  segmented exclusive scan of delta[vals[j]] in key order over L levels (lvl_n[0] = ne; level l >= 1 has
 //                lvl_n[l] items and its lvl_agg / lvl_out / lvl_head; lvl_out[0] receives the scan, lvl_head[0] the heads)
+//   zk_bal_prefix_sum  exclusive prefix sum of n > 0 uint32 counters in place (totals: 1024 words of workspace); also
+//                serves assets.cu, which numbers its segments with it
 namespace zkbal { struct Pair; }
+int zk_bal_prefix_sum(zk_ctx *ctx, uint32_t *c, size_t n, uint32_t *totals);
 int zk_bal_sort(zk_ctx *ctx, size_t ne, size_t n_acct, uint32_t *keys0, uint32_t *keys1, uint32_t *vals0, uint32_t *vals1, uint32_t *hist,
                 uint32_t *totals, const uint32_t **keys, const uint32_t **vals);
 int zk_bal_scan(zk_ctx *ctx, const uint32_t *keys, const uint32_t *vals, const zkbal::Pair *delta, size_t L, const size_t *lvl_n,

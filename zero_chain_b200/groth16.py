@@ -779,6 +779,212 @@ def import_anonymous_block(ctx: Context, pvk: PreparedVerifyingKey, accounts, tx
     return verdicts, (host[oo[3]:oo[4]], host[oo[4]:oo[5]], host[oo[5]:oo[6]]), host[oo[0]:oo[1]]
 
 
+# ---- encrypted-asset calls of one block (modules/encrypted-assets/src/lib.rs:32-215, 266-358) -----------------------------
+# zk_assets_block kinds; statuses as BLOCK_*, slot flags as ACCOUNT_*
+ASSET_TRANSFER, ASSET_ISSUE, ASSET_DESTROY = 0, 1, 2
+ASSET_ID_MAX = 2**32 - 1            # AssetId = u32 (runtime/src/lib.rs)
+
+
+def assets_block(ctx: Context, balances, pendings, flags, kind, slot_a, slot_b, tx_points, applied):
+    """confidential_transfer, issue and destroy over a block of (AssetId, EncKey) slots, in order (zk_assets_block).
+    balances / pendings: 64 bytes per slot; flags: one ACCOUNT_* byte per slot; kind: one ASSET_* byte per transaction;
+    slot_a: the sender's / issuer's (new id, issuer) / owner's slot; slot_b: the recipient's slot (transfers only);
+    tx_points: 128 bytes per transaction (transfer: amount_sender | amount_recipient | fee_sender | randomness; issue: total
+    | - | - | randomness); applied: one byte per transaction, applied when 1.  Returns (balance_sender, balance_after,
+    event_ct, event_flags, status, new_balances, new_pendings, new_flags) as bytes; balance_after, event_ct and event_flags
+    are zero where the call writes nothing.  Raises SynthesisError(ZK_ERR_DECODE) naming the slot when a named slot's
+    stored ciphertext does not read."""
+    n_slots, n_tx = len(flags), len(kind)
+    bal, pend, fl, kd, tp, ap = (_cat(balances, 64), _cat(pendings, 64), bytes(flags), bytes(kind), _cat(tx_points, 128), bytes(applied))
+    assert len(bal) == len(pend) == 64 * n_slots and len(slot_a) == len(slot_b) == n_tx and len(tp) == 128 * n_tx and len(ap) == n_tx
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    idx = lambda v: np.ascontiguousarray(np.asarray(v, np.int64).astype(np.uint32)) if n_tx else np.zeros(1, np.uint32)
+    z = lambda n: np.zeros(max(n, 1), np.uint8)
+    bs, ba, ev, ef, st = z(64 * n_tx), z(64 * n_tx), z(128 * n_tx), z(n_tx), z(n_tx)
+    nb, npd, nf = z(64 * n_slots), z(64 * n_slots), z(n_slots)
+    _ck(_lib.lib().zk_assets_block(ctx._h, n_slots, _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n_tx, _p(buf(kd)), _p(idx(slot_a)),
+                                   _p(idx(slot_b)), _p(buf(tp)), _p(buf(ap)), _p(bs), _p(ba), _p(ev), _p(ef), _p(st), _p(nb), _p(npd), _p(nf)))
+    return (bs[:64 * n_tx].tobytes(), ba[:64 * n_tx].tobytes(), ev[:128 * n_tx].tobytes(), ef[:n_tx].tobytes(), st[:n_tx].tobytes(),
+            nb[:64 * n_slots].tobytes(), npd[:64 * n_slots].tobytes(), nf[:n_slots].tobytes())
+
+
+def assets_block_device(ctx: Context, n_slots: int, d_balances_ptr: int, d_pendings_ptr: int, d_flags_ptr: int, n_tx: int, d_kind_ptr: int,
+                        d_slot_a_ptr: int, d_slot_b_ptr: int, d_tx_points_ptr: int, d_applied_ptr: int, d_balance_sender_ptr: int,
+                        d_balance_after_ptr: int, d_event_ct_ptr: int, d_event_flags_ptr: int, d_status_ptr: int, d_new_balances_ptr: int,
+                        d_new_pendings_ptr: int, d_new_flags_ptr: int):
+    """The same on device pointers (d_slot_a / d_slot_b: uint32), asynchronous on the context's stream; ctx.sync() raises
+    SynthesisError(ZK_ERR_DECODE) naming a named slot whose stored ciphertext did not read.  Only the applied transactions'
+    entries of d_balance_after (transfers) and d_event_ct / d_event_flags (issues and destroys) are written."""
+    v = lambda x: C.c_void_p(x) if x else None
+    _ck(_lib.lib().zk_assets_block_device(ctx._h, n_slots, v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr), n_tx, v(d_kind_ptr),
+                                          v(d_slot_a_ptr), v(d_slot_b_ptr), v(d_tx_points_ptr), v(d_applied_ptr), v(d_balance_sender_ptr),
+                                          v(d_balance_after_ptr), v(d_event_ct_ptr), v(d_event_flags_ptr), v(d_status_ptr),
+                                          v(d_new_balances_ptr), v(d_new_pendings_ptr), v(d_new_flags_ptr)))
+
+
+class AssetTransferTx:
+    """One confidential_transfer extrinsic of encrypted-assets (lib.rs:86-99): its accounts are the slots (asset_id,
+    address_sender) and (asset_id, address_recipient); rvk is the signer, g_epoch the block's LastGEpoch."""
+    kind = ASSET_TRANSFER
+
+    def __init__(self, asset_id: int, address_sender, address_recipient, amount_sender, amount_recipient, fee_sender, randomness,
+                 rvk, g_epoch, nonce):
+        self.asset_id = int(asset_id)
+        self.address_sender, self.address_recipient = _pt32(address_sender), _pt32(address_recipient)
+        self.amount_sender, self.amount_recipient = _pt32(amount_sender), _pt32(amount_recipient)
+        self.fee_sender, self.randomness = _pt32(fee_sender), _pt32(randomness)
+        self.rvk, self.g_epoch, self.nonce = _pt32(rvk), _pt32(g_epoch), _pt32(nonce)
+
+    def points(self) -> bytes:
+        return self.amount_sender + self.amount_recipient + self.fee_sender + self.randomness
+
+    def verify_points(self, balance_sender: bytes) -> bytes:
+        return confidential_points(self.address_sender, self.address_recipient, self.amount_sender, self.amount_recipient,
+                                   self.randomness, self.fee_sender, balance_sender, self.rvk, self.g_epoch, self.nonce)
+
+
+class IssueTx:
+    """One issue extrinsic (lib.rs:32-41): the new asset's slot is (NextAssetId, issuer)."""
+    kind = ASSET_ISSUE
+
+    def __init__(self, issuer, total, fee, balance, randomness, rvk, g_epoch, nonce):
+        self.issuer, self.total, self.fee = _pt32(issuer), _pt32(total), _pt32(fee)
+        self.balance, self.randomness = _ct64(balance), _pt32(randomness)
+        self.rvk, self.g_epoch, self.nonce = _pt32(rvk), _pt32(g_epoch), _pt32(nonce)
+
+    def points(self) -> bytes:
+        return self.total + bytes(64) + self.randomness
+
+    def verify_points(self) -> bytes:
+        """what lib.rs:53-64 passes: (issuer, issuer, total, total, balance, rvk, fee, randomness, nonce)"""
+        return confidential_points(self.issuer, self.issuer, self.total, self.total, self.randomness, self.fee, self.balance, self.rvk,
+                                   self.g_epoch, self.nonce)
+
+
+class DestroyTx:
+    """One destroy extrinsic (lib.rs:167-177) of the slot (asset_id, owner)."""
+    kind = ASSET_DESTROY
+
+    def __init__(self, owner, asset_id: int, dummy_amount, dummy_fee, dummy_balance, randomness, rvk, g_epoch, nonce):
+        self.owner, self.asset_id = _pt32(owner), int(asset_id)
+        self.dummy_amount, self.dummy_fee, self.dummy_balance = _pt32(dummy_amount), _pt32(dummy_fee), _ct64(dummy_balance)
+        self.randomness, self.rvk, self.g_epoch, self.nonce = _pt32(randomness), _pt32(rvk), _pt32(g_epoch), _pt32(nonce)
+
+    def points(self) -> bytes:
+        return bytes(128)
+
+    def verify_points(self) -> bytes:
+        """what lib.rs:188-199 passes: (owner, owner, dummy_amount, dummy_amount, dummy_balance, rvk, dummy_fee, randomness,
+        nonce)"""
+        return confidential_points(self.owner, self.owner, self.dummy_amount, self.dummy_amount, self.randomness, self.dummy_fee,
+                                   self.dummy_balance, self.rvk, self.g_epoch, self.nonce)
+
+
+def import_assets_block(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
+    """Verify and apply a block of encrypted-asset extrinsics the way the runtime does, one after another.  state =
+    (slots, balances, pendings, flags): slots lists the (asset_id, enc_key) of each row of the slot table, the rest as
+    assets_block takes them; txs: AssetTransferTx / IssueTx / DestroyTx list; proofs: 192 bytes each; next_asset_id: the
+    NextAssetId before the block; new_slot_flags: the flags of a slot the block creates (ACCOUNT_DUE when current_epoch >
+    0, since its LastRollOver is absent).
+
+    Issue and destroy proofs read only extrinsic fields, so they are verified first, in one batch.  The passing issues are
+    numbered from next_asset_id, which names their slots.  Every (asset_id, key) is then resolved to a slot; new ones are
+    appended, absent.  A transfer's proof reads its sender's balance, which depends on the sender slot's earlier transfers
+    that passed (issues and destroys are decided by then), so the transfers take the rounds of import_confidential_block,
+    with chains keyed by sender slot: at most 1 + (the most failures in one chain), one when nothing fails.
+
+    Returns (verdicts, asset_ids, events, (slots, new_balances, new_pendings, new_flags), rounds): the reference's verdict
+    per transaction (1 passes; the other values as verify_proofs_with_points); the id each passing issue created (None
+    elsewhere); the event ciphertexts of each applied transaction (a transfer: the sender's balance after; an issue: the
+    total, also its TotalSupply; a destroy: (taken balance, taken pending), b"" for an absent one, as Ciphertext::default())
+    and None for the others.  Raises ValueError when an asset id would pass 2^32 - 1, SynthesisError(ZK_ERR_DECODE) for a
+    named slot whose stored ciphertext does not read."""
+    slots, balances, pendings, flags = state
+    slots = [(int(a), _pt32(k)) for a, k in slots]
+    n = len(txs)
+    proofs = _cat(proofs, 192)
+    assert len(proofs) == 192 * n and len(flags) == len(slots)
+    proof_rows = np.frombuffer(proofs, np.uint8).reshape(n, 192) if n else np.zeros((0, 192), np.uint8)
+    kinds = np.array([t.kind for t in txs], np.uint8)
+    verdicts = np.full(n, -1, np.int16)                      # -1: undecided
+    fixed = np.flatnonzero(kinds != ASSET_TRANSFER)
+    if len(fixed):
+        pts = b"".join(txs[k].verify_points() for k in fixed.tolist())
+        verdicts[fixed] = verify_proofs_with_points(pvk, proof_rows[fixed].tobytes(), pts, CONFIDENTIAL_POINTS)
+    # asset ids, then slots
+    index = {s: i for i, s in enumerate(slots)}
+    bal, pend, fl = bytearray(_cat(balances, 64)), bytearray(_cat(pendings, 64)), bytearray(flags)
+
+    def slot(asset_id, key):
+        s = (asset_id, key)
+        if s not in index:
+            index[s] = len(slots)
+            slots.append(s)
+            bal.extend(bytes(64)); pend.extend(bytes(64)); fl.append(new_slot_flags & 0xFF & ~(ACCOUNT_BALANCE | ACCOUNT_PENDING))
+        return index[s]
+    asset_ids = [None] * n
+    next_id = int(next_asset_id)
+    none = 0xFFFFFFFF                                         # past every slot: a failed issue or destroy touches nothing
+    slot_a, slot_b = np.full(n, none, np.uint32), np.full(n, none, np.uint32)
+    for k, t in enumerate(txs):
+        if t.kind == ASSET_ISSUE:
+            if verdicts[k] != 1:
+                continue
+            if next_id > ASSET_ID_MAX:
+                raise ValueError("import_assets_block: asset id %d would pass 2^32 - 1" % next_id)
+            asset_ids[k] = next_id
+            slot_a[k] = slot(next_id, t.issuer)
+            next_id += 1
+        elif t.kind == ASSET_DESTROY:
+            if verdicts[k] == 1:
+                slot_a[k] = slot(t.asset_id, t.owner)
+        else:
+            slot_a[k] = slot(t.asset_id, t.address_sender)
+            slot_b[k] = slot(t.asset_id, t.address_recipient)
+    tx_points = b"".join(t.points() for t in txs)
+    table = (bytes(bal), bytes(pend), bytes(fl))
+    is_transfer = kinds == ASSET_TRANSFER
+    chains = None
+    rounds = 0
+    while True:
+        mask = np.where(is_transfer, (verdicts == -1) | (verdicts == 1), verdicts == 1).astype(np.uint8)
+        out = assets_block(ctx, *table, kinds.tobytes(), slot_a, slot_b, tx_points, mask.tobytes())
+        undecided = np.flatnonzero(verdicts == -1)
+        if not len(undecided):
+            break
+        rounds += 1
+        bs = out[0]
+        pts = b"".join(txs[k].verify_points(bs[64 * k:64 * k + 64]) for k in undecided.tolist())
+        got = np.array(verify_proofs_with_points(pvk, proof_rows[undecided].tobytes(), pts, CONFIDENTIAL_POINTS), np.int16)
+        if (got == 1).all():
+            verdicts[undecided] = 1
+            break                   # every balance of this round was exact: out is the final state
+        if chains is None:
+            chains = {}
+            for k in np.flatnonzero(is_transfer).tolist():
+                chains.setdefault(int(slot_a[k]), []).append(k)
+        got_of = dict(zip(undecided.tolist(), got.tolist()))
+        for chain in chains.values():
+            for k in chain:
+                if verdicts[k] != -1:
+                    continue
+                verdicts[k] = got_of[k]
+                if got_of[k] != 1:
+                    break
+    events = [None] * n
+    ba, ev, ef, st = out[1], out[2], out[3], out[4]
+    for k in range(n):
+        if st[k] != BLOCK_APPLIED:
+            continue
+        if kinds[k] == ASSET_TRANSFER:
+            events[k] = ba[64 * k:64 * k + 64]
+        elif kinds[k] == ASSET_ISSUE:
+            events[k] = ev[128 * k:128 * k + 64]
+        else:
+            events[k] = tuple(ev[128 * k + 64 * w:128 * k + 64 * w + 64] if ef[k] >> w & 1 else b"" for w in range(2))
+    return [int(v) for v in verdicts], asset_ids, events, (slots,) + out[5:], rounds
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96
