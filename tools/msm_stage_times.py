@@ -11,6 +11,9 @@ seeded scalars) and prints one JSON line:
   setup, accumulate, tail) from a separate blocking run under torch.profiler (CUDA activities).  `rounds` also gives each
   round's wall span and how much of its forward and invert time lay under a running backward pass (0 while a round's
   kernels run one after another on one stream);
+- `byte_model`: for every round's forward and backward pass, the DRAM bytes per pair the code has to move (a MODEL worked out
+  from the kernels, not a measurement), the round's pair count estimated from the shape, and the effective GB/s those bytes
+  make over the measured kernel time;
 - the card's name and power limit.
 The profiled runs' chrome traces are written to DIR (a new temporary directory if --out is not given).
 """
@@ -106,6 +109,52 @@ def breakdown(events):
     return {k: v / n / 1e3 for k, v in sorted(parts.items())}, out_rounds, len(msms)
 
 
+FQ = 48                        # bytes of an Fq element; a G1 affine point is 2 FQ
+SECTOR = 32                    # DRAM / L2 sector
+
+
+def sectors(nbytes, offset=0):
+    """Bytes moved at sector granularity for nbytes at a random address with the given offset within a sector."""
+    return ((offset + nbytes + SECTOR - 1) // SECTOR) * SECTOR
+
+
+def byte_model(n, window_bits, rounds):
+    """DRAM bytes per pair of each batched-affine pass (msm_batchaff.cuh), from the data layout, and the pair counts of the
+    rounds estimated from the shape: E = n W entries (zero digits ignored), each round pairs half of its inputs and keeps one
+    odd leftover in about half of the 2^(c-1) buckets.  Round 1 gathers window-table rows (x | y, 96-byte rows, so a row starts
+    on a sector) at random; later rounds read the previous round's x and y planes in order.  Per pair:
+      forward   round 1: two entry codes (8) + two x gathers (2 x 64 at sector granularity) + prefix store (48)
+                round r>1: two x (96) + prefix store (48)
+      backward  round 1: two entry codes (8) + two row gathers (2 x 96) + prefix (48) + the sum's x and y stored (96)
+                round r>1: two points (192) + prefix (48) + the sum's x and y stored (96)
+    The bucket offsets are read once per bucket crossed and are left out."""
+    W = 255 // window_bits + 1
+    nb = 1 << (window_bits - 1)
+    entries, out = float(n * W), {}
+    for r in range(1, rounds + 1):
+        pairs = entries / 2 - nb / 4
+        if r == 1:
+            fwd = 8 + 2 * sectors(FQ) + FQ
+            bwd = 8 + 2 * sectors(2 * FQ) + FQ + 2 * FQ
+        else:
+            fwd = 2 * FQ + FQ
+            bwd = 2 * 2 * FQ + FQ + 2 * FQ
+        out["round%d" % r] = {"entries": entries, "pairs": pairs, "forward_bytes_per_pair": fwd, "backward_bytes_per_pair": bwd}
+        entries = pairs + nb / 2           # outputs: the pairs' sums and the odd leftovers
+    return out
+
+
+def with_rates(model, parts):
+    """Adds each pass's modelled bytes and the effective GB/s over its measured time (kernels_ms, per MSM)."""
+    for rnd, m in model.items():
+        for p in ("forward", "backward"):
+            ms = parts.get("%s.%s" % (rnd, p))
+            m["%s_model_bytes" % p] = m["pairs"] * m["%s_bytes_per_pair" % p]
+            m["%s_ms" % p] = ms
+            m["%s_effective_GBps" % p] = m["%s_model_bytes" % p] / (ms * 1e-3) / 1e9 if ms else None
+    return model
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="directory for the profiler traces (default: a new temporary directory)")
@@ -179,12 +228,13 @@ def main():
         prof.export_chrome_trace(traces[what])
 
     parts, rounds, n_msm = breakdown(kernel_events(traces["blocking"]))
+    model = with_rates(byte_model(n, bases.window_bits, len(rounds)), parts)
     by_name = {}
     for name, t0, t1 in kernel_events(traces["in_flight"]):
         by_name[short(name)] = by_name.get(short(name), 0.0) + (t1 - t0) / args.steps / 1e3
     line = {"label": args.label, "log_n": args.log_n, "window_bits": bases.window_bits, "steps": args.steps,
             "blocking_ms": blocking_ms, "in_flight_ms": in_flight_ms,
-            "stage_ms": stage_ms / max(1, launches), "kernels_ms": parts, "rounds": rounds, "profiled_msms": n_msm,
+            "stage_ms": stage_ms / max(1, launches), "kernels_ms": parts, "rounds": rounds, "byte_model": model, "profiled_msms": n_msm,
             "in_flight_kernels_ms": dict(sorted(by_name.items(), key=lambda kv: -kv[1])),
             "card": card(), "traces": traces}
     with open(os.path.join(out, "%s.json" % args.label), "w") as f:

@@ -55,7 +55,7 @@ extern "C" void zk_ctx_destroy(zk_ctx *c) {
     DevBuf *bufs[] = {&c->scalars, &c->digits, &c->tile_hist, &c->tile_off, &c->sizes, &c->bucket_off, &c->task_off, &c->scan_scratch,
                       &c->sorted, &c->partials, &c->buckets, &c->red_part, &c->red_x, &c->result, &c->out_bytes, &c->stage_a, &c->stage_b,
                       &c->stage_c, &c->ntt_tmp, &c->g_a, &c->g_b, &c->g_c, &c->g_h, &c->g_scal, &c->g_misc,
-                      &c->aff_pts0, &c->aff_pts1, &c->aff_scratch, &c->aff_off0, &c->aff_off1, &c->aff_sizes0, &c->aff_sizes1, &c->aff_srcs, &c->aff_tot, &c->red_rows, &c->g_scal2, &c->g_scal3, &c->sorted2, &c->coarse_off, &c->coarse_sizes, &c->task_order, &c->len_hist, &c->heavy_list, &c->red_tmp,
+                      &c->aff_pts0, &c->aff_pts1, &c->aff_scratch, &c->aff_off0, &c->aff_off1, &c->aff_sizes0, &c->aff_sizes1, &c->aff_tot, &c->red_rows, &c->g_scal2, &c->g_scal3, &c->sorted2, &c->coarse_off, &c->coarse_sizes, &c->task_order, &c->len_hist, &c->heavy_list, &c->red_tmp,
                       &c->v_pts, &c->v_stat, &c->v_coef, &c->v_f, &c->v_part, &c->v_io, &c->v_jj,
                       &c->eg_table, &c->eg_index, &c->jm, &c->bal, &c->bal_io};
     for (DevBuf *b : bufs) b->release();

@@ -67,7 +67,7 @@ struct zk_ctx {
     int sm_count = 0;
     int *d_err = nullptr;          // device error flag (non-canonical scalar etc.)
     // MSM workspace
-    DevBuf aff_pts0, aff_pts1, aff_scratch, aff_off0, aff_off1, aff_sizes0, aff_sizes1, aff_srcs, aff_tot;   // batched-affine rounds (msm_batchaff.cuh)
+    DevBuf aff_pts0, aff_pts1, aff_scratch, aff_off0, aff_off1, aff_sizes0, aff_sizes1, aff_tot;   // batched-affine rounds (msm_batchaff.cuh)
     DevBuf scalars, digits, tile_hist, tile_off, sizes, bucket_off, task_off, scan_scratch, sorted, partials, buckets, red_part, red_x, red_rows, sorted2, coarse_off, coarse_sizes, task_order, len_hist, heavy_list, red_tmp, result, out_bytes;
     bool len_hist_zeroed = false;
     // generic staging

@@ -21,8 +21,10 @@ __device__ __forceinline__ Affine<F> load_affine(const Affine<F> *__restrict__ p
     return r;
 }
 // MINB = minimum resident blocks per SM (register budget: 2 -> <=255 regs, 3 -> 168, 4 -> 128)
+// Points: ys == nullptr -> xs holds affine rows x | y (row r: x = xs[2r], y = xs[2r + 1]: bases or window tables); otherwise
+// two planes x = xs[i], y = ys[i] (the last batched-affine round's outputs, msm_batchaff.cuh).
 template <class F, int MINB>
-__global__ void __launch_bounds__(128, MINB) k_accumulate(const Affine<F> *__restrict__ bases, const uint32_t *__restrict__ sorted,
+__global__ void __launch_bounds__(128, MINB) k_accumulate(const F *__restrict__ xs, const F *__restrict__ ys, const uint32_t *__restrict__ sorted,
                                                     const uint32_t *__restrict__ bucket_off, const uint32_t *__restrict__ task_off,
                                                     uint32_t n_buckets, const uint32_t *__restrict__ order, XYZZ<F> *__restrict__ partials) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -44,15 +46,18 @@ __global__ void __launch_bounds__(128, MINB) k_accumulate(const Affine<F> *__res
     // The next point is prefetched with cp.async into a per-thread shared-memory slot while the current mixed
     // addition runs: the gather latency is hidden without holding a second point (24+ registers) live.
     // sorted == nullptr: the inputs are already-reduced affine points indexed by position (no sign)
-    constexpr int VEC = (int)(sizeof(Affine<F>) / 16);
+    constexpr int VEC = (int)(sizeof(Affine<F>) / 16), FV = (int)(sizeof(F) / 16);
     __shared__ uint4 stage[128 * VEC];
     uint4 *slot = stage + threadIdx.x * VEC;
     const uint32_t slot_addr = (uint32_t)__cvta_generic_to_shared(slot);
     auto prefetch = [&](uint32_t c) {
-        const uint4 *src = reinterpret_cast<const uint4 *>(bases + (c & 0x7fffffffu));
+        const F *px = ys ? xs + c : xs + 2 * (size_t)(c & 0x7fffffffu), *py = ys ? ys + c : px + 1;
+        const uint4 *sx = reinterpret_cast<const uint4 *>(px), *sy = reinterpret_cast<const uint4 *>(py);
 #pragma unroll
-        for (int k = 0; k < VEC; k++)
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(slot_addr + 16u * k), "l"(src + k) : "memory");
+        for (int k = 0; k < FV; k++) {
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(slot_addr + 16u * k), "l"(sx + k) : "memory");
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(slot_addr + 16u * (FV + k)), "l"(sy + k) : "memory");
+        }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
     uint32_t code = sorted ? sorted[e0] : e0;

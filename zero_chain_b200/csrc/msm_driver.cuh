@@ -101,7 +101,8 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
     //     (zk_ctx_set_opt), and the
     //     number of rounds follows the average bucket length (the host knows the upper bound E / NB; sparse scalars make the
     //     rounds cheaper, not wrong).
-    const Affine<F> *cur_pts = (const Affine<F> *)b->d_tbl;
+    // the points of the next pass: the window tables (rows x | y), then each round's outputs as an x plane and a y plane
+    const F *cur_x = (const F *)b->d_tbl, *cur_y = nullptr;
     const uint32_t *cur_sorted = ctx->sorted.as<uint32_t>(), *cur_off = ctx->bucket_off.as<uint32_t>(), *cur_sizes = ctx->sizes.as<uint32_t>();
     // zk_ctx_profile: the bucket-accumulation stage (affine rounds, if any, + the XYZZ pass); destroyed here unless handed to the context
     struct ProfPair {
@@ -144,9 +145,9 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
             const size_t T_total = (size_t)grid * BA_T;
             DevBuf *pts_o = pts_buf[l & 1], *off_o = off_buf[l & 1], *sz_o = sz_buf[l & 1];
             ZK_TRY(pts_o->reserve(out_max * sizeof(Affine<F>)));
+            F *out_x = pts_o->as<F>(), *out_y = out_x + out_max;        // x plane, then y plane
             ZK_TRY(off_o->reserve((NB + 1) * 4)); ZK_TRY(sz_o->reserve((NB + 1) * 4));
             ZK_TRY(ctx->aff_scratch.reserve((size_t)(K + 1) * T_total * sizeof(F)));
-            ZK_TRY(ctx->aff_srcs.reserve(out_max * sizeof(uint2)));
             const size_t n_tot = (size_t)grid * (BA_T / 32);            // one total per warp
             ZK_TRY(ctx->aff_tot.reserve(3 * n_tot * sizeof(F)));
             F *tot = ctx->aff_tot.as<F>(), *tot_scr = tot + n_tot, *tot_inv = tot + 2 * n_tot;
@@ -154,21 +155,19 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
             exclusive_scan<false>(sz_o->as<uint32_t>(), off_o->as<uint32_t>(), NB, ctx->scan_scratch.as<uint32_t>(), st);
             const uint32_t *off_out = off_o->as<uint32_t>();
             if (l == 0)
-                k_ba_forward<F, true><<<grid, BA_T, ba_smem_forward<F>(), st>>>(cur_pts, cur_sorted, cur_off, off_out, (uint32_t)NB, K, ctx->aff_scratch.as<F>(),
-                                                                               ctx->aff_srcs.as<uint2>(), tot);
+                k_ba_forward<F, true><<<grid, BA_T, ba_smem_forward<F>(), st>>>(cur_x, cur_y, cur_sorted, cur_off, off_out, (uint32_t)NB, K, ctx->aff_scratch.as<F>(), tot);
             else
-                k_ba_forward<F, false><<<grid, BA_T, ba_smem_forward<F>(), st>>>(cur_pts, nullptr, cur_off, off_out, (uint32_t)NB, K, ctx->aff_scratch.as<F>(),
-                                                                                ctx->aff_srcs.as<uint2>(), tot);
+                k_ba_forward<F, false><<<grid, BA_T, ba_smem_forward<F>(), st>>>(cur_x, cur_y, nullptr, cur_off, off_out, (uint32_t)NB, K, ctx->aff_scratch.as<F>(), tot);
             k_ba_invert<F><<<1, BA_INV_T, ba_smem_invert<F>(), st>>>(tot, off_out, (uint32_t)NB, K, tot_scr, tot_inv);
             const int Kb = K;
-#define ZK_BA_BWD(FIRST_, MB_) k_ba_backward<F, FIRST_, MB_><<<grid, BA_T, ba_smem_backward<F>(), st>>>(cur_pts, off_out, (uint32_t)NB, Kb, ctx->aff_scratch.as<F>(), \
-                                                                                                    ctx->aff_srcs.as<uint2>(), tot_inv, pts_o->as<Affine<F>>())
+#define ZK_BA_BWD(FIRST_, MB_) k_ba_backward<F, FIRST_, MB_><<<grid, BA_T, ba_smem_backward<F>(), st>>>(cur_x, cur_y, cur_sorted, cur_off, off_out, (uint32_t)NB, Kb, \
+                                                                                                    ctx->aff_scratch.as<F>(), tot_inv, out_x, out_y)
 #ifdef ZK_EXPERIMENTS
             if (minb == 3) { if (l == 0) ZK_BA_BWD(true, 3); else ZK_BA_BWD(false, 3); } else
 #endif
             { if (l == 0) ZK_BA_BWD(true, BA_MINB); else ZK_BA_BWD(false, BA_MINB); }
 #undef ZK_BA_BWD
-            cur_pts = pts_o->as<Affine<F>>(); cur_sorted = nullptr;
+            cur_x = out_x; cur_y = out_y; cur_sorted = nullptr;
             cur_off = off_out; cur_sizes = sz_o->as<uint32_t>();
             in_max = out_max;
         }
@@ -198,11 +197,10 @@ int msm_run_t(zk_ctx *ctx, const zk_bases *b, const uint32_t *d_scalars, size_t 
         }
     }
     {
-        const Affine<F> *tb = cur_pts;
         const uint32_t *so = cur_sorted, *bo = cur_off, *to = ctx->task_off.as<uint32_t>();
         unsigned grid = (unsigned)((t_max + 127) / 128);
         if (ctx->prof_on && !ev0) { cudaEventCreate(&ev0); cudaEventCreate(&ev1); cudaEventRecord(ev0, st); }
-        k_accumulate<F, 3><<<grid, 128, 0, st>>>(tb, so, bo, to, (uint32_t)NB, order, partials);      // 3 CTAs / SM (168 registers, no spills)
+        k_accumulate<F, 3><<<grid, 128, 0, st>>>(cur_x, cur_y, so, bo, to, (uint32_t)NB, order, partials);      // 3 CTAs / SM (168 registers, no spills)
     }
     if (ctx->prof_on) { cudaEventRecord(ev1, st); ctx->prof_events.push_back(ev0); ctx->prof_events.push_back(ev1); prof.kept = true; }
     if (ctx->split_tail) {             // asynchronous MSM: combine / reduction continue on the high-priority tail stream
