@@ -103,3 +103,10 @@ void emu_fq_mul_sub_mul(const uint32_t *a, const uint32_t *b, const uint32_t *c,
     Fq r = zkwide::mul_sub_mul(x, y, z, w); memcpy(o, r.l, 48);
 }
 }
+
+// ---- the scalar split of k_scale_points (glv_split.cuh): n scalars of 8 words -> k0 | k1, 4 words each
+#include <stddef.h>
+#include "glv_split.cuh"
+extern "C" void emu_glv_split_many(const uint32_t *k, size_t n, uint32_t *out) {
+    for (size_t i = 0; i < n; i++) zkglv::split_u2(k + 8 * i, out + 8 * i, out + 8 * i + 4);
+}

@@ -118,3 +118,25 @@ def test_separated_multiply_reduce_emulation(emu):
         assert _call(emu, "emu_fq_mul_sep", n, a, b) == a * b * rinv % mod
         assert _call(emu, "emu_fq_sqr_sep", n, a) == a * a * rinv % mod
         assert _call(emu, "emu_fq_mul_sub_mul", n, a, b, c, d) == (a * b - c * d) * rinv % mod
+
+
+def test_glv_split_emulation(emu):
+    """glv_split.cuh: k = k1 u^2 + k0 by shift-and-subtract, as k_scale_points runs it on one thread, against divmod for the
+    GLV edge scalars (tests/prove_forge.py) and 10^5 random scalars below 2^255."""
+    from tests import prove_forge as pf
+    rng = np.random.Generator(np.random.Philox(31))
+    words = rng.integers(0, 1 << 32, size=(100000, 8), dtype=np.uint64).astype(np.uint32)
+    words[:, 7] &= 0x7FFFFFFF
+    words[::3, 7] &= 0x73EDA753                        # a third of them below r, like every canonical blinding scalar
+    edges = list(pf.GLV_EDGES.values()) + [0, 1, pr.R - 1, (1 << 255) - 1]
+    edge_words = np.array([[(k >> (32 * i)) & 0xFFFFFFFF for i in range(8)] for k in edges], np.uint32)
+    k = np.ascontiguousarray(np.concatenate([edge_words, words]))
+    out = np.zeros((k.shape[0], 8), np.uint32)
+    emu.emu_glv_split_many(k.ctypes.data_as(C.c_void_p), C.c_size_t(k.shape[0]), out.ctypes.data_as(C.c_void_p))
+    as_int = lambda row: sum(int(x) << (32 * i) for i, x in enumerate(row))
+    bad = []
+    for i in range(k.shape[0]):
+        kk = as_int(k[i])
+        if (as_int(out[i, :4]), as_int(out[i, 4:])) != pf.glv_split(kk):
+            bad.append(hex(kk))
+    assert bad[:5] == []

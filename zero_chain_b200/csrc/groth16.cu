@@ -19,6 +19,7 @@
 #include "internal.h"
 #include "codec.cuh"
 #include "curve_coop.cuh"
+#include "glv_split.cuh"
 
 struct zk_params {
     int device = 0;
@@ -356,21 +357,7 @@ __global__ void __launch_bounds__(SCALE_T) k_scale_points(const G1XYZZ *__restri
         if (t == 0) pw[0] = d;
         for (int i = 1; i <= top; i++) { zkcoop::dbl(d); if (t == 0) pw[i] = d; }
     } else if (glv && t == 32) {                                                // meanwhile, on the other warp: k = k1 * u^2 + k0 by shift-and-subtract
-        const uint32_t dv[4] = {0x00000000u, 0x00000001u, 0x0001a402u, 0xac45a401u};        // u^2 = 0xd201000000010000^2
-        uint32_t rem[5] = {0, 0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
-        for (int i = 254; i >= 0; i--) {
-            for (int w = 4; w > 0; w--) rem[w] = (rem[w] << 1) | (rem[w - 1] >> 31);
-            rem[0] = (rem[0] << 1) | ((k[i >> 5] >> (i & 31)) & 1);
-            bool ge = rem[4] != 0;
-            if (!ge) { ge = true; for (int w = 3; w >= 0; w--) { if (rem[w] != dv[w]) { ge = rem[w] > dv[w]; break; } } }
-            if (ge) {
-                uint64_t br = 0;
-                for (int w = 0; w < 4; w++) { uint64_t x = (uint64_t)rem[w] - dv[w] - br; rem[w] = (uint32_t)x; br = (x >> 63) & 1; }
-                rem[4] -= (uint32_t)br;
-                if (i < 128) q[i >> 5] |= 1u << (i & 31);
-            }
-        }
-        for (int w = 0; w < 4; w++) { kk[0][w] = rem[w]; kk[1][w] = q[w]; }
+        zkglv::split_u2(k, kk[0], kk[1]);
     }
     __syncthreads();
     G1XYZZ acc = G1XYZZ::inf();

@@ -228,12 +228,12 @@ static int get_tables(zk_ctx *ctx, unsigned log_n, NttSlot **out) {
 //   log_n <= 11          one rows pass, the whole vector in one shared-memory tile (in place)
 //   12 <= log_n <= 22    columns pass data -> tmp, rows pass tmp -> data
 //   log_n > 22           outer split N = 2^(log_n-22) x 2^22: columns pass over the outer dimension, then every 2^22 row
-//                        gets the two passes above with the root w^(2^(log_n-22)) and a transposed final store (batch == 1)
+//                        gets the two passes above with the root w^(2^(log_n-22)) and a transposed final store; a batch runs
+//                        these three passes once per vector (grid.y already indexes the rows), all through the one ntt_tmp
 int zk_ntt_run(zk_ctx *ctx, void *d_data, unsigned log_n, int mode, size_t batch) {
     if (log_n > 32) { zk_set_error("PolynomialDegreeTooLarge: log_n = %u", log_n); return ZK_ERR_POLY_DEGREE_TOO_LARGE; }
     if (log_n > 28) { zk_set_error("NTT sizes above 2^28 are not supported by this build (twiddle tables would need %llu GB)", (unsigned long long)(96ull << (log_n - 30))); return ZK_ERR_INVALID; }
     if (mode < 0 || mode > 3 || batch == 0 || batch > 65535) { zk_set_error("zk_ntt: bad mode/batch"); return ZK_ERR_INVALID; }
-    if (log_n > 2 * MAX_TILE_LOG && batch != 1) { zk_set_error("batched NTTs above 2^22 are not supported"); return ZK_ERR_INVALID; }
     ZK_TRY(zk_use_device(ctx));
     if (log_n == 0) return ZK_OK;     // size-1 transform is the identity (m^-1 = 1)
     NttSlot *t;
@@ -276,10 +276,13 @@ int zk_ntt_run(zk_ctx *ctx, void *d_data, unsigned log_n, int mode, size_t batch
         Fr *tmp = ctx->ntt_tmp.as<Fr>();
         const int l0 = (int)log_n - 2 * MAX_TILE_LOG;                       // outer dimension 2^l0 <= 2^10
         PassGeom g0{log_n, log_n, l0, 0, 0, 0};
-        cols(data, tmp, g0, 1, coset_in);                                   // outer columns, twiddle w^(n' m0)
         PassGeom g1{log_n, 2 * MAX_TILE_LOG, MAX_TILE_LOG, l0, 1, l0};
-        cols(tmp, tmp, g1, 1u << l0, 0);                                    // every row: inner columns (in place)
-        rows(tmp, data, g1, 1u << l0, 0, post);                             // every row: inner rows, store at m0 + 2^l0 * m'
+        for (size_t b = 0; b < batch; b++) {                                // in stream order: vector b + 1 reuses tmp after b is done
+            Fr *v = data + b * n;
+            cols(v, tmp, g0, 1, coset_in);                                  // outer columns, twiddle w^(n' m0)
+            cols(tmp, tmp, g1, 1u << l0, 0);                                // every row: inner columns (in place)
+            rows(tmp, v, g1, 1u << l0, 0, post);                            // every row: inner rows, store at m0 + 2^l0 * m'
+        }
     }
     ZK_CUDA(cudaGetLastError());
     return ZK_OK;
