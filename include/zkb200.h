@@ -378,6 +378,43 @@ int zk_balances_anonymous_block_device(zk_ctx *ctx, size_t n_accounts, const uin
                                        const uint8_t *d_tx_points, const uint8_t *d_tx_extra, const uint8_t *d_g_epoch,
                                        const uint8_t *d_applied, uint8_t *d_enc_balances, uint8_t *d_verify_points, uint8_t *d_tx_status,
                                        uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags);
+/* ---- both calls of modules/anonymous-balances in one block ---------------------------------------------------------------
+ * anonymous_transfer and issue (modules/anonymous-balances/src/lib.rs:23-134) for n_tx transactions in block order: the
+ * arguments of zk_balances_anonymous_block, plus
+ * kind[k]: 0 anonymous_transfer, 1 issue.  An issue uses members[12 k] as its issuer (the other 11 entries are ignored),
+ *   slot 0 of its tx_points row as total and slot 12 as randomness (the other slots are ignored); its tx_extra row is
+ *   ignored.  The caller builds an issue's 11 verifier points from its extrinsic fields (verify_confidential_proof over
+ *   (issuer, issuer, total, total, balance, rvk, fee, randomness, nonce)) and checks it with the confidential key.
+ * issued[k]: 64 B, the Issued event's ciphertext from_left_right(total, randomness) as Point::write encodings; written for
+ *   applied issues only, other entries are left as they are.
+ * An applied issue sets the issuer's balance to that ciphertext and touches nothing else: no rollover, the pending balance
+ *   and the due bit stay.  So the balance a transfer reads for member m is the last applied issue to m after m's first
+ *   transfer touch and before the transfer, else m's rolled balance, where the rollover at the first touch starts from the
+ *   last applied issue before it (or the stored balance).  The final balance follows the same rule at the end of the block.
+ * tx_status[k]: as zk_balances_anonymous_block for a transfer.  An issue: 3 the issuer >= n_accounts, or an unknown kind; 2
+ *   total or randomness fails Point::read + as_prime_order; 1 not applied (applied[k] != 1); 0 applied.  3 comes before 2
+ *   and 2 before 1.  An issue's and an unknown kind's enc_balances and verify_points rows are zero bytes.
+ * new_balances / new_pendings / new_flags: as zk_balances_anonymous_block.  An account only issues name is never decoded:
+ *   without an applied issue it is copied through byte for byte; with one, its balance is the last issued encoding, its
+ *   pending bytes are copied, and its flags gain bit 0 (bit 2 stays).
+ * ZK_ERR_DECODE as zk_balances_anonymous_block: an account a transfer touches must have stored ciphertexts that read, even
+ *   when an issue before the touch replaces the stored balance.  ZK_ERR_INVALID as zk_balances_anonymous_block, and for a
+ *   NULL kind or issued when n_tx > 0.  With no issue and no unknown kind the outputs are zk_balances_anonymous_block's. */
+#define ZK_ANON_TRANSFER 0
+#define ZK_ANON_ISSUE 1
+int zk_anonymous_calls_block(zk_ctx *ctx, size_t n_accounts, const uint8_t *keys, const uint8_t *balances, const uint8_t *pendings,
+                             const uint8_t *acct_flags, size_t n_tx, const uint8_t *kind, const uint32_t *members, const uint8_t *tx_points,
+                             const uint8_t *tx_extra, const uint8_t *g_epoch, const uint8_t *applied, uint8_t *enc_balances,
+                             uint8_t *verify_points, uint8_t *issued, uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings,
+                             uint8_t *new_flags);
+/* the same with device pointers (d_members 4-byte aligned); asynchronous on the context's stream.  A touched account that
+ * fails to decode is reported by the next zk_ctx_sync as ZK_ERR_DECODE, with the account named in zk_last_error */
+int zk_anonymous_calls_block_device(zk_ctx *ctx, size_t n_accounts, const uint8_t *d_keys, const uint8_t *d_balances,
+                                    const uint8_t *d_pendings, const uint8_t *d_acct_flags, size_t n_tx, const uint8_t *d_kind,
+                                    const uint32_t *d_members, const uint8_t *d_tx_points, const uint8_t *d_tx_extra,
+                                    const uint8_t *d_g_epoch, const uint8_t *d_applied, uint8_t *d_enc_balances, uint8_t *d_verify_points,
+                                    uint8_t *d_issued, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
+                                    uint8_t *d_new_flags);
 /* ---- encrypted-asset calls of one block (what modules/encrypted-assets runs around each proof) --------------------------
  * confidential_transfer, issue and destroy (modules/encrypted-assets/src/lib.rs:32-215, 266-358) for n_tx transactions, in
  * order, over a table of n_slots slots: one slot per (AssetId, EncKey), numbered by the caller.

@@ -81,6 +81,8 @@ SIGNATURES = {
     "zk_balances_confidential_block_device": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_anonymous_block": (i32, [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_anonymous_block_device": (i32, [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "zk_anonymous_calls_block": (i32, [vp, sz, vp, vp, vp, vp, sz] + [vp] * 13),
+    "zk_anonymous_calls_block_device": (i32, [vp, sz, vp, vp, vp, vp, sz] + [vp] * 13),
     "zk_assets_block": (i32, [vp, sz, vp, vp, vp, sz] + [vp] * 13),
     "zk_assets_block_device": (i32, [vp, sz, vp, vp, vp, sz] + [vp] * 13),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),

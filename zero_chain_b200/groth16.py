@@ -711,9 +711,13 @@ def anonymous_block_device(ctx: Context, n_accounts: int, d_keys_ptr: int, d_bal
                                                       v(d_new_balances_ptr), v(d_new_pendings_ptr), v(d_new_flags_ptr)))
 
 
+ANON_TRANSFER, ANON_ISSUE = 0, 1    # zk_anonymous_calls_block kinds
+
+
 class AnonymousTx:
     """One anonymous_transfer extrinsic (lib.rs:23-30) with its ring as indices into the block's account table: the 12
     members (enc_keys), their left ciphertexts, right_ciphertext, the signer's rvk and the nonce."""
+    kind = ANON_TRANSFER
 
     def __init__(self, members, left_ciphertexts, right_ciphertext, rvk, nonce):
         self.members = [int(m) for m in members]
@@ -727,20 +731,91 @@ class AnonymousTx:
         return b"".join(self.left_ciphertexts) + self.right_ciphertext
 
 
-def import_anonymous_block(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
-    """Verify and apply a block of anonymous transfers the way the runtime does, with the state, the verifier's inputs and
-    the verdicts on the device.  accounts = (keys, balances, pendings, flags) as anonymous_block takes them; txs:
-    AnonymousTx list; g_epoch: the block's 32-byte LastGEpoch; proofs: 192 bytes each.
+def anonymous_calls_block(ctx: Context, keys, balances, pendings, flags, kind, members, tx_points, tx_extra, g_epoch, applied):
+    """anonymous_transfer and issue in block order (zk_anonymous_calls_block): the arguments of anonymous_block plus kind,
+    one ANON_* byte per transaction.  An issue's issuer is its members[0] (the other 11 are ignored), its total slot 0 and
+    its randomness slot 12 of its tx_points row; its tx_extra row is ignored.  Returns (enc_balances, verify_points,
+    issued, status, new_balances, new_pendings, new_flags) as bytes: issued holds 64 bytes per transaction, the Issued
+    ciphertext of each applied issue and zero bytes elsewhere; an issue's enc_balances and verify_points rows are zero.
+    Raises SynthesisError(ZK_ERR_DECODE) as anonymous_block."""
+    n_acct = len(flags)
+    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1).astype(np.uint32))
+    assert len(mem) % ANONIMITY_SIZE == 0
+    n_tx = len(mem) // ANONIMITY_SIZE
+    ky, bal, pend, fl, kd = _cat(keys, 32), _cat(balances, 64), _cat(pendings, 64), bytes(flags), bytes(kind)
+    tp, tx, ge, ap = _cat(tx_points, 32 * (ANONIMITY_SIZE + 1)), _cat(tx_extra, 64), _pt32(g_epoch), bytes(applied)
+    assert len(ky) == 32 * n_acct and len(bal) == len(pend) == 64 * n_acct and len(kd) == n_tx
+    assert len(tp) == 32 * (ANONIMITY_SIZE + 1) * n_tx and len(tx) == 64 * n_tx and len(ap) == n_tx
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    z = lambda n: np.zeros(max(n, 1), np.uint8)
+    eb, vp, iss, st = z(64 * ANONIMITY_SIZE * n_tx), z(32 * ANONYMOUS_POINTS * n_tx), z(64 * n_tx), z(n_tx)
+    nb, npd, nf = z(64 * n_acct), z(64 * n_acct), z(n_acct)
+    _ck(_lib.lib().zk_anonymous_calls_block(ctx._h, n_acct, _p(buf(ky)), _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n_tx, _p(buf(kd)),
+                                            _p(mem if n_tx else np.zeros(1, np.uint32)), _p(buf(tp)), _p(buf(tx)), _p(buf(ge)), _p(buf(ap)),
+                                            _p(eb), _p(vp), _p(iss), _p(st), _p(nb), _p(npd), _p(nf)))
+    return (eb[:64 * ANONIMITY_SIZE * n_tx].tobytes(), vp[:32 * ANONYMOUS_POINTS * n_tx].tobytes(), iss[:64 * n_tx].tobytes(),
+            st[:n_tx].tobytes(), nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes())
 
-    A transfer changes pending balances only, so what each proof is checked against (its members' balances after their
-    rollover) does not depend on any verdict.  One upload, then: anonymous_block_device with nothing applied gives every
-    transaction's 52 public-input points; verify_proofs_with_points_device checks the proofs on them; anonymous_block_device
-    again, with the verdict buffer as the mask, gives the final state; one download.
 
-    Returns (verdicts, (new_balances, new_pendings, new_flags), enc_balances): the reference's verdict per transaction (1
-    passes; the other values as verify_proofs_with_points) and the 12 balances (768 bytes) each transaction's proof was
-    checked against.  Raises ValueError for an account index out of range, SynthesisError(ZK_ERR_DECODE) for a touched
-    account whose stored ciphertext does not read."""
+def anonymous_calls_block_device(ctx: Context, n_accounts: int, d_keys_ptr: int, d_balances_ptr: int, d_pendings_ptr: int,
+                                 d_flags_ptr: int, n_tx: int, d_kind_ptr: int, d_members_ptr: int, d_tx_points_ptr: int, d_tx_extra_ptr: int,
+                                 d_g_epoch_ptr: int, d_applied_ptr: int, d_enc_balances_ptr: int, d_verify_points_ptr: int,
+                                 d_issued_ptr: int, d_status_ptr: int, d_new_balances_ptr: int, d_new_pendings_ptr: int,
+                                 d_new_flags_ptr: int):
+    """The same on device pointers (d_members: uint32), asynchronous on the context's stream; only the applied issues'
+    entries of d_issued are written.  ctx.sync() raises SynthesisError(ZK_ERR_DECODE) as anonymous_block_device."""
+    v = lambda x: C.c_void_p(x) if x else None
+    _ck(_lib.lib().zk_anonymous_calls_block_device(ctx._h, n_accounts, v(d_keys_ptr), v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr),
+                                                   n_tx, v(d_kind_ptr), v(d_members_ptr), v(d_tx_points_ptr), v(d_tx_extra_ptr),
+                                                   v(d_g_epoch_ptr), v(d_applied_ptr), v(d_enc_balances_ptr), v(d_verify_points_ptr),
+                                                   v(d_issued_ptr), v(d_status_ptr), v(d_new_balances_ptr), v(d_new_pendings_ptr),
+                                                   v(d_new_flags_ptr)))
+
+
+class AnonIssueTx:
+    """One issue extrinsic of anonymous-balances (lib.rs:87-99): issuer is an index into the block's account table; rvk is
+    the signer."""
+    kind = ANON_ISSUE
+
+    def __init__(self, issuer: int, total, fee, balance, randomness, rvk, nonce):
+        self.issuer = int(issuer)
+        self.total, self.fee, self.balance, self.randomness = _pt32(total), _pt32(fee), _ct64(balance), _pt32(randomness)
+        self.rvk, self.nonce = _pt32(rvk), _pt32(nonce)
+
+    @property
+    def members(self):
+        return [self.issuer] * ANONIMITY_SIZE
+
+    def points(self) -> bytes:
+        return self.total + bytes(32 * (ANONIMITY_SIZE - 1)) + self.randomness
+
+    def verify_points(self, keys, g_epoch) -> bytes:
+        """what lib.rs:111-122 passes to verify_confidential_proof: (issuer, issuer, total, total, balance, rvk, fee,
+        randomness, nonce); keys: the account table's EncKeys"""
+        ky = _cat(keys, 32)
+        issuer = ky[32 * self.issuer:32 * self.issuer + 32]
+        return confidential_points(issuer, issuer, self.total, self.total, self.randomness, self.fee, self.balance, self.rvk,
+                                   _pt32(g_epoch), self.nonce)
+
+
+def import_anonymous_calls_block(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, accounts, txs, g_epoch,
+                                 proofs):
+    """Verify and apply a block of anonymous-balances extrinsics (AnonymousTx and AnonIssueTx, in block order) the way the
+    runtime does, with the state, the verifier's inputs and the verdicts on the device.  accounts = (keys, balances,
+    pendings, flags) as anonymous_block takes them; g_epoch: the block's 32-byte LastGEpoch; proofs: 192 bytes each,
+    checked with conf_pvk for issues and anon_pvk for transfers.
+
+    An issue's proof reads only its own fields, and a transfer changes pending balances only, so nothing a proof is checked
+    against depends on a transfer's verdict.  One upload, then: the issues' proofs on their 11 points; the state pass with
+    the issue verdicts as the mask (no transfer applied), which gives every transfer's 52 public-input points; the
+    transfers' proofs on them; the state pass again with all the verdicts; one download.  A block without issues takes
+    zk_balances_anonymous_block's passes.
+
+    Returns (verdicts, (new_balances, new_pendings, new_flags), enc_balances, issued): the reference's verdict per
+    transaction (1 passes; the other values as verify_proofs_with_points), the 12 balances (768 bytes, zero for an issue)
+    each transfer's proof was checked against, and the Issued ciphertext (64 bytes) of each applied issue, None
+    elsewhere.  Raises ValueError for an account index out of range, SynthesisError(ZK_ERR_DECODE) for a touched account
+    whose stored ciphertext does not read."""
     import torch
     keys, balances, pendings, flags = accounts
     n_acct, n = len(flags), len(txs)
@@ -751,32 +826,85 @@ def import_anonymous_block(ctx: Context, pvk: PreparedVerifyingKey, accounts, tx
     ky, bal, pend, fl, ge = _cat(keys, 32), _cat(balances, 64), _cat(pendings, 64), bytes(flags), _pt32(g_epoch)
     assert len(ky) == 32 * n_acct and len(bal) == len(pend) == 64 * n_acct
     if not n:
-        return [], (bal, pend, fl), b""
+        return [], (bal, pend, fl), b"", []
+    kind = np.array([t.kind for t in txs], np.uint8)
+    iss_idx, tr_idx = np.flatnonzero(kind == ANON_ISSUE), np.flatnonzero(kind == ANON_TRANSFER)
+    n_iss, n_tr = len(iss_idx), len(tr_idx)
     members = np.array([t.members for t in txs], np.uint32).reshape(-1)
-    # one host buffer of the inputs (members first, 4-byte aligned), one of the outputs; each one transfer
-    parts = [members.tobytes(), ky, bal, pend, fl, b"".join(t.points() for t in txs), b"".join(t.rvk + t.nonce for t in txs), ge, proofs]
+    proof_rows = np.frombuffer(proofs, np.uint8).reshape(n, 192)
+    iss_points = b"".join(txs[k].verify_points(ky, ge) for k in iss_idx.tolist())
+    idx = np.concatenate([iss_idx, tr_idx]).astype(np.int64)
+    # one host buffer of the inputs (members and the index lists first, 4- and 8-byte aligned), one of the outputs
+    parts = [idx.tobytes(), members.tobytes(), ky, bal, pend, fl, b"".join(t.points() for t in txs),
+             b"".join(t.rvk + t.nonce for t in txs),
+             ge, kind.tobytes(), proof_rows[iss_idx].tobytes(), proof_rows[tr_idx].tobytes(), iss_points]
     offs = np.cumsum([0] + [len(p) for p in parts]).tolist()
     dev = torch.device("cuda", ctx.device)
     d_in = torch.frombuffer(bytearray(b"".join(parts)), dtype=torch.uint8).to(dev)
-    sizes = [64 * ANONIMITY_SIZE * n, 32 * ANONYMOUS_POINTS * n, n, 64 * n_acct, 64 * n_acct, n_acct, n, n]
+    sizes = [64 * ANONIMITY_SIZE * n, 32 * ANONYMOUS_POINTS * n, 64 * n, n, 64 * n_acct, 64 * n_acct, n_acct, n, n]
     oo = np.cumsum([0] + sizes).tolist()
-    d_out = torch.zeros(oo[-1], dtype=torch.uint8, device=dev)     # the last n bytes: the all-zero mask of the first call
+    d_out = torch.zeros(oo[-1], dtype=torch.uint8, device=dev)     # the last 2n bytes: the mask, then the compact verdicts
     torch.cuda.current_stream(dev).synchronize()                    # the context's stream is not torch's
     pi = lambda i: d_in.data_ptr() + offs[i]
     po = lambda i: d_out.data_ptr() + oo[i]
-    state = lambda applied: anonymous_block_device(ctx, n_acct, pi(1), pi(2), pi(3), pi(4), n, pi(0), pi(5), pi(6), pi(7), applied,
-                                                   po(0), po(1), po(2), po(3), po(4), po(5))
-    state(po(7))
-    if pvk.ctx is not ctx:
-        ctx.sync()
-    verify_proofs_with_points_device(pvk, n, pi(8), po(1), ANONYMOUS_POINTS, po(6))
-    if pvk.ctx is not ctx:
-        pvk.ctx.sync()
-    state(po(6))
+    d_idx = d_in[offs[0]:offs[1]].view(torch.int64)
+    mask, compact = d_out[oo[7]:oo[8]], d_out[oo[8]:oo[9]]
+    rows = d_out[oo[1]:oo[2]].view(n, 32 * ANONYMOUS_POINTS)
+    ctx_stream = torch.cuda.ExternalStream(ctx.stream, device=dev) if ctx.stream else torch.cuda.default_stream(dev)
+
+    def sync_pvk(pvk):
+        if pvk.ctx is not ctx:
+            ctx.sync()
+        return pvk
+
+    def done_pvk(pvk):
+        if pvk.ctx is not ctx:
+            pvk.ctx.sync()
+
+    def state():
+        if n_iss:
+            anonymous_calls_block_device(ctx, n_acct, pi(2), pi(3), pi(4), pi(5), n, pi(9), pi(1), pi(6), pi(7), pi(8), po(7), po(0), po(1),
+                                         po(2), po(3), po(4), po(5), po(6))
+        else:
+            anonymous_block_device(ctx, n_acct, pi(2), pi(3), pi(4), pi(5), n, pi(1), pi(6), pi(7), pi(8), po(7), po(0), po(1), po(3),
+                                   po(4), po(5), po(6))
+    if n_iss:
+        verify_proofs_with_points_device(sync_pvk(conf_pvk), n_iss, pi(10), pi(12), CONFIDENTIAL_POINTS, po(8))
+        done_pvk(conf_pvk)
+        with torch.cuda.stream(ctx_stream):
+            mask.index_copy_(0, d_idx[:n_iss], compact[:n_iss])
+    state()
+    if n_tr:
+        with torch.cuda.stream(ctx_stream):
+            tr_rows = rows.index_select(0, d_idx[n_iss:]) if n_iss else rows
+        # without issues the verdicts land in the mask directly
+        verify_proofs_with_points_device(sync_pvk(anon_pvk), n_tr, pi(11), tr_rows.data_ptr(), ANONYMOUS_POINTS,
+                                         po(8) + n_iss if n_iss else po(7))
+        done_pvk(anon_pvk)
+        if n_iss:
+            with torch.cuda.stream(ctx_stream):
+                mask.index_copy_(0, d_idx[n_iss:], compact[n_iss:])
+        state()
     ctx.sync()
-    host = d_out[:oo[7]].cpu().numpy().tobytes()
-    verdicts = [int(v) for v in host[oo[6]:oo[7]]]
-    return verdicts, (host[oo[3]:oo[4]], host[oo[4]:oo[5]], host[oo[5]:oo[6]]), host[oo[0]:oo[1]]
+    host = d_out[:oo[8]].cpu().numpy().tobytes()
+    verdicts = [int(v) for v in host[oo[7]:oo[8]]]
+    st = host[oo[3]:oo[4]]
+    issued = [host[oo[2] + 64 * k:oo[2] + 64 * k + 64] if kind[k] == ANON_ISSUE and st[k] == BLOCK_APPLIED else None for k in range(n)]
+    return verdicts, (host[oo[4]:oo[5]], host[oo[5]:oo[6]], host[oo[6]:oo[7]]), host[oo[0]:oo[1]], issued
+
+
+def import_anonymous_block(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
+    """Verify and apply a block of anonymous transfers the way the runtime does, with the state, the verifier's inputs and
+    the verdicts on the device: import_anonymous_calls_block for a block without issues.  accounts = (keys, balances,
+    pendings, flags) as anonymous_block takes them; txs: AnonymousTx list; g_epoch: the block's 32-byte LastGEpoch;
+    proofs: 192 bytes each.
+
+    Returns (verdicts, (new_balances, new_pendings, new_flags), enc_balances): the reference's verdict per transaction (1
+    passes; the other values as verify_proofs_with_points) and the 12 balances (768 bytes) each transaction's proof was
+    checked against.  Raises ValueError for an account index out of range, SynthesisError(ZK_ERR_DECODE) for a touched
+    account whose stored ciphertext does not read."""
+    verdicts, state, enc_balances, _ = import_anonymous_calls_block(ctx, pvk, None, accounts, txs, g_epoch, proofs)
+    return verdicts, state, enc_balances
 
 
 # ---- encrypted-asset calls of one block (modules/encrypted-assets/src/lib.rs:32-215, 266-358) -----------------------------
