@@ -462,6 +462,66 @@ int zk_assets_block_device(zk_ctx *ctx, size_t n_slots, const uint8_t *d_balance
                            const uint8_t *d_applied, uint8_t *d_balance_sender, uint8_t *d_balance_after, uint8_t *d_event_ct,
                            uint8_t *d_event_flags, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
                            uint8_t *d_new_flags);
+/* ---- block import: the proofs and the state of encrypted-balances / encrypted-assets transfers in one call ----------------
+ * A transfer's proof is checked against the sender's balance at that transaction, which depends on which of the sender's
+ * earlier transfers passed.  So the call runs rounds: every transfer starts undecided and counts as applied; each round
+ * runs the state pass with the current mask, verifies the undecided transfers against the balance_sender it gives
+ * (zk_groth16_verify_points_batch with 11 points), and in each chain (the transfers of one sender) decides the undecided
+ * transfers up to and including the first whose verdict is not 1; the rest waits for the next round.  A round without a
+ * failure ends the import with its state pass; a round that leaves nothing undecided is followed by one last state pass.
+ * A block takes 1 + (the most failures in one chain) rounds at most, one fewer when those failures end the chain, and one
+ * when nothing fails; a block without transfers takes none.
+ *
+ * zk_import_confidential_block: the arguments of zk_balances_confidential_block, with the verifier's inputs in place of
+ *   tx_points and applied.
+ * rows: n_tx * 11 * 32 B, each transfer's verifier points in verify_confidential_proof's push order (address_sender,
+ *   address_recipient, amount_sender, amount_recipient, randomness, fee_sender, balance_sender left, balance_sender right,
+ *   rvk, g_epoch, nonce).  Slots 6-7 are ignored: the call fills them from the state.  The state pass's tx_points are
+ *   slots 2, 3, 5, 4.
+ * proofs: n_tx * 192 B.  pvk: a prepared key of 11-point proofs on the context's device, ready to use.
+ * verdicts[k]: the verdict of transaction k, as zk_groth16_verify_points_batch gives it (1 passes).
+ * balance_after, tx_status, new_balances, new_pendings, new_flags: zk_balances_confidential_block's outputs for the final
+ *   mask; balance_after is zero for a transaction that is not applied.
+ * rounds: the number of verification launches (may be NULL).
+ * ZK_ERR_INVALID, naming the lowest such transaction in zk_last_error, when a sender or recipient is >= n_accounts; and as
+ *   zk_balances_confidential_block for NULL arguments and sizes.  ZK_ERR_MALFORMED_VK for a key of other than 11 points.
+ *   ZK_ERR_DECODE as zk_balances_confidential_block; the outputs are then undefined. */
+int zk_import_confidential_block(zk_ctx *ctx, const zk_pvk *pvk, size_t n_accounts, const uint8_t *balances, const uint8_t *pendings,
+                                 const uint8_t *acct_flags, size_t n_tx, const uint32_t *sender, const uint32_t *recipient,
+                                 const uint8_t *rows, const uint8_t *proofs, uint8_t *verdicts, uint8_t *balance_after, uint8_t *tx_status,
+                                 uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags, unsigned *rounds);
+/* the same with device pointers (d_sender / d_recipient 4-byte aligned; rounds is a host pointer).  The call blocks on the
+ * context's stream before the first round and after each round, to read a block of four counters, and returns with the
+ * outputs complete; it reports ZK_ERR_DECODE itself. */
+int zk_import_confidential_block_device(zk_ctx *ctx, const zk_pvk *pvk, size_t n_accounts, const uint8_t *d_balances,
+                                        const uint8_t *d_pendings, const uint8_t *d_acct_flags, size_t n_tx, const uint32_t *d_sender,
+                                        const uint32_t *d_recipient, const uint8_t *d_rows, const uint8_t *d_proofs, uint8_t *d_verdicts,
+                                        uint8_t *d_balance_after, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
+                                        uint8_t *d_new_flags, unsigned *rounds);
+/* zk_import_assets_block: the transfer rounds over zk_assets_block, with chains keyed by the sender slot (slot_a).  The
+ *   arguments of zk_assets_block, with rows, proofs and fixed_verdicts in place of applied.  Asset ids and slots are the
+ *   caller's, as for zk_assets_block: they depend on the issue verdicts, which the caller has before the call.
+ * rows / proofs: as zk_import_confidential_block, read at transfers only.
+ * fixed_verdicts[k]: the verdict of issue or destroy k: 1 passes and is applied, any other byte fails; ignored at transfers.
+ * verdicts[k]: fixed_verdicts[k] for an issue or destroy, byte for byte, the transfer's verdict otherwise.  verdicts may be
+ *   the fixed_verdicts buffer itself.
+ * balance_after, event_ct, event_flags, tx_status, new_balances, new_pendings, new_flags: zk_assets_block's outputs for the
+ *   final mask, with zero bytes where it writes nothing.
+ * ZK_ERR_INVALID, naming the lowest such transaction, for an unknown kind, a transfer's slot_a or slot_b >= n_slots, or a
+ *   passing issue's or destroy's slot_a >= n_slots (a failing one's slots are ignored); otherwise as
+ *   zk_import_confidential_block. */
+int zk_import_assets_block(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const uint8_t *balances, const uint8_t *pendings,
+                           const uint8_t *slot_flags, size_t n_tx, const uint8_t *kind, const uint32_t *slot_a, const uint32_t *slot_b,
+                           const uint8_t *tx_points, const uint8_t *rows, const uint8_t *proofs, const uint8_t *fixed_verdicts,
+                           uint8_t *verdicts, uint8_t *balance_after, uint8_t *event_ct, uint8_t *event_flags, uint8_t *tx_status,
+                           uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags, unsigned *rounds);
+/* the same with device pointers, blocking as zk_import_confidential_block_device does */
+int zk_import_assets_block_device(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const uint8_t *d_balances, const uint8_t *d_pendings,
+                                  const uint8_t *d_slot_flags, size_t n_tx, const uint8_t *d_kind, const uint32_t *d_slot_a,
+                                  const uint32_t *d_slot_b, const uint8_t *d_tx_points, const uint8_t *d_rows, const uint8_t *d_proofs,
+                                  const uint8_t *d_fixed_verdicts, uint8_t *d_verdicts, uint8_t *d_balance_after, uint8_t *d_event_ct,
+                                  uint8_t *d_event_flags, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
+                                  uint8_t *d_new_flags, unsigned *rounds);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

@@ -1,0 +1,155 @@
+#!/usr/bin/env python3
+"""Measures block import with the verify / apply rounds, and prints one JSON line:
+  - the card's name and power limit, read in this run;
+  - for a block of --conf-tx confidential transfers over --accounts accounts, and one of --asset-tx encrypted-asset calls
+    (transfers, with --issue-frac issues and --destroy-frac destroys) over --slots slots, alternated in one process, median
+    of --reps, wall clock around calls that end in a stream synchronise:
+      driver   the Python drivers import_confidential_block / import_assets_block (a state call from host buffers and a
+               verification launch per round, the rounds assembled in numpy)
+      call     the one C call, confidential_import / assets_import (zk_import_confidential_block / zk_import_assets_block:
+               one upload, the rounds on the device, one download; assets_import verifies the issues and destroys first)
+      verify   verify_proofs_with_points_device alone on every proof of the block, on device-resident points
+  - the rounds, and the ratios call / verify and driver / verify.
+--fail-rate is the fraction of transfers (and of issues and destroys) whose proof fails; a transfer after a failure in its
+chain is proven against the balance without it, so each failure costs a round.  Proofs are forged from a toy key's
+trapdoor (tests/import_corpus.py, 22 public inputs: the verifier does the work of the real key per proof).  Every output
+of every timed call is checked inside the run: the driver's and the call's equal, and the final state, balance_after,
+events and verdicts equal the C oracle's (balances_oracle.c, assets_oracle.c) for the intended verdicts.  Nothing is
+written to the repository."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from tests import import_corpus as ic                     # noqa: E402
+from zero_chain_b200 import groth16 as zk                  # noqa: E402
+
+
+def log(*a):
+    print(*a, file=sys.stderr, flush=True)                 # progress: the corpus and the C oracle take minutes
+
+
+def card():
+    try:
+        out = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], text=True)
+        name, power = [s.strip() for s in out.strip().split("\n")[0].split(",")]
+        return name, power
+    except Exception as e:                                 # the numbers are still printed, with the reason
+        return "unknown (%s)" % e, "unknown"
+
+
+def timed(fn):
+    import torch
+    torch.cuda.synchronize()
+    t = time.perf_counter()
+    out = fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t) * 1e3, out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--conf-tx", type=int, default=8192)
+    ap.add_argument("--accounts", type=int, default=1024)
+    ap.add_argument("--asset-tx", type=int, default=4096)
+    ap.add_argument("--slots", type=int, default=1024)
+    ap.add_argument("--issue-frac", type=float, default=0.05)
+    ap.add_argument("--destroy-frac", type=float, default=0.02)
+    ap.add_argument("--fail-rate", type=float, default=0.01)
+    ap.add_argument("--skew", type=float, default=1.0)
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--seed", type=int, default=7)
+    a = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("import_bench: no CUDA device (the measurement runs on the GPU only)")
+    name, power = card()
+    ctx = zk.Context(0)
+    key = ic.ForgeKey(5)
+    pvk = zk.PreparedVerifyingKey.prepare(ctx, key.params_bytes)
+    res = {"card": name, "power_limit": power, "fail_rate": a.fail_rate, "reps": a.reps}
+    dev = torch.device("cuda", 0)
+
+    def verify_alone(rows, proofs):
+        n = len(proofs)
+        d_rows = torch.frombuffer(bytearray(rows), dtype=torch.uint8).to(dev)
+        d_proofs = torch.frombuffer(bytearray(b"".join(proofs)), dtype=torch.uint8).to(dev)
+        d_out = torch.zeros(n, dtype=torch.uint8, device=dev)
+        torch.cuda.synchronize()
+
+        def run():
+            zk.verify_proofs_with_points_device(pvk, n, d_proofs.data_ptr(), d_rows.data_ptr(), zk.CONFIDENTIAL_POINTS, d_out.data_ptr())
+            ctx.sync()
+            return d_out.cpu().numpy().tobytes()
+        return run
+
+    def measure(label, driver, call, verify, check):
+        for fn in (driver, call, verify):            # warm-up: module loads, workspace growth
+            fn()
+        times = {"driver": [], "call": [], "verify": []}
+        for r in range(a.reps):
+            for k, fn in (("driver", driver), ("call", call), ("verify", verify)):
+                ms, out = timed(fn)
+                times[k].append(ms)
+                check(k, out)
+            log(label, "rep", r, {k: round(v[-1], 2) for k, v in times.items()})
+        med = {k: float(np.median(v)) for k, v in times.items()}
+        return {"ms": {k: round(v, 3) for k, v in med.items()}, "call_over_verify": round(med["call"] / med["verify"], 3),
+                "driver_over_verify": round(med["driver"] / med["verify"], 3)}
+
+    # ---- confidential transfers
+    log("confidential corpus: %d transfers over %d accounts" % (a.conf_tx, a.accounts))
+    blk = ic.confidential(key, a.accounts, a.conf_tx, a.seed, fail_frac=a.fail_rate, skew=a.skew,
+                          state_call=lambda *x: zk.confidential_block(ctx, *x))
+    want = zk.confidential_import(ctx, pvk, blk.accounts, blk.txs, blk.proofs)
+    log("C oracle (confidential)")
+    o = blk.oracle(want[0])
+    assert want[0] == blk.intended, "verdicts differ from the intended ones"
+    assert (o[0],) + o[2:] == (want[2],) + want[1], "the import differs from the C oracle"
+    v_want = bytes(want[0])
+
+    def check_conf(k, out):
+        if k == "verify":
+            assert out == v_want, "verification alone differs"
+        else:
+            assert out == want, "%s differs" % k
+    res["confidential"] = dict(measure("confidential", lambda: zk.import_confidential_block(ctx, pvk, blk.accounts, blk.txs, blk.proofs),
+                                       lambda: zk.confidential_import(ctx, pvk, blk.accounts, blk.txs, blk.proofs),
+                                       verify_alone(blk.rows, blk.proofs), check_conf),
+                               n_tx=a.conf_tx, accounts=a.accounts, rounds=want[3], failures=sum(v != 1 for v in want[0]))
+
+    # ---- encrypted-asset calls
+    log("asset corpus: %d calls over %d slots" % (a.asset_tx, a.slots))
+    ab = ic.assets(key, a.slots, a.asset_tx, a.seed + 1, fail_frac=a.fail_rate, fixed_fail_frac=a.fail_rate, issue_frac=a.issue_frac,
+                   destroy_frac=a.destroy_frac, skew=a.skew, state_call=lambda *x: zk.assets_block(ctx, *x))
+    awant = zk.assets_import(ctx, pvk, *ab.args())
+    log("C oracle (assets)")
+    ao = ab.oracle(awant[0])
+    assert awant[0] == ab.intended, "asset verdicts differ from the intended ones"
+    assert awant[3][1:] == ao[5:], "the asset import differs from the C oracle"
+    assert all(awant[2][k] == ao[1][64 * k:64 * k + 64] for k, t in enumerate(ab.txs) if t.kind == zk.ASSET_TRANSFER and ao[4][k] == 0)
+    av_want = bytes(awant[0])
+
+    def check_assets(k, out):
+        if k == "verify":
+            assert out == av_want, "verification alone differs"
+        else:
+            assert out == awant, "%s differs" % k
+    res["assets"] = dict(measure("assets", lambda: zk.import_assets_block(ctx, pvk, *ab.args()), lambda: zk.assets_import(ctx, pvk, *ab.args()),
+                                 verify_alone(ab.rows, ab.proofs), check_assets),
+                         n_tx=a.asset_tx, slots=a.slots, rounds=awant[4], failures=sum(v != 1 for v in awant[0]))
+    res["outputs_equal_oracle"] = True
+    pvk.free()
+    ctx.close()
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()

@@ -85,6 +85,10 @@ SIGNATURES = {
     "zk_anonymous_calls_block_device": (i32, [vp, sz, vp, vp, vp, vp, sz] + [vp] * 13),
     "zk_assets_block": (i32, [vp, sz, vp, vp, vp, sz] + [vp] * 13),
     "zk_assets_block_device": (i32, [vp, sz, vp, vp, vp, sz] + [vp] * 13),
+    "zk_import_confidential_block": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 10 + [C.POINTER(u32)]),
+    "zk_import_confidential_block_device": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 10 + [C.POINTER(u32)]),
+    "zk_import_assets_block": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 15 + [C.POINTER(u32)]),
+    "zk_import_assets_block_device": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 15 + [C.POINTER(u32)]),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),
 }
 

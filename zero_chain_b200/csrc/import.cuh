@@ -1,0 +1,147 @@
+// The verify / apply rounds of a block import (import.cu): zk_import_confidential_block and zk_import_assets_block.
+//
+// A transfer's proof is checked against the sender's balance at that transaction, and that balance depends on which of
+// the sender's earlier transfers passed.  So every transfer starts undecided and counts as applied, and each round
+//   1. runs the state pass (zk_balances_confidential_block / zk_assets_block) with the current mask,
+//   2. compacts the undecided transfers (imp_flag, zk_bal_prefix_sum, imp_gather): their proofs, and their 11 verifier
+//      points with slots 6-7 (balance_sender) taken from the state pass,
+//   3. verifies the compacted rows (zk_groth16_verify_points_batch_device),
+//   4. finds each chain's first failure (imp_fail: atomicMin over the failing rows) and decides every undecided transfer
+//      up to and including it (imp_decide): the balances those read were exact.  The rest waits for the next round.
+// A chain is the transfers of one key: the sender account, or the sender slot.  The undecided transfers of a chain are
+// always a suffix of it, so "up to the first failure" is "k <= first_fail[key]".  A round without a failure decides every
+// undecided transfer as passed, and its state pass is the final state; a round that leaves nothing undecided is followed
+// by one last state pass.  Issues and destroys (zk_import_assets_block) carry the caller's verdicts from the start.
+//
+// Plain integer code, one function per item and thread of each pass; the same source compiles with ZK_HOST_EMUL for the
+// CPU test (tests/host_emul/emul_import.cpp), which runs the rounds as loops over the items.
+#pragma once
+#include <stddef.h>
+#include <stdint.h>
+
+#ifdef ZK_HOST_EMUL
+#define ZK_IMP_DEV inline
+#else
+#define ZK_IMP_DEV __device__ __forceinline__
+#endif
+
+namespace zkimp {
+
+constexpr uint8_t IMP_UNDECIDED = 0xFF;        // a transfer's verdict not known yet (the verifier's verdicts are 0..4)
+constexpr uint32_t IMP_NONE = 0xFFFFFFFFu;
+constexpr uint8_t IMP_TRANSFER = 0;            // zk_assets_block's kinds
+constexpr uint8_t IMP_DESTROY = 2;
+constexpr int IMP_POINTS = 11;                 // confidential_points: address_sender, address_recipient, amount_sender,
+                                               // amount_recipient, randomness, fee_sender, balance_sender (2), rvk, g_epoch, nonce
+constexpr int IMP_ROW = 32 * IMP_POINTS;       // bytes of a verifier row
+constexpr int IMP_BS = 32 * 6;                 // offset of balance_sender in it
+constexpr int IMP_WORDS = (IMP_ROW + 192) / 4; // 4-byte words of a row and a proof, gathered one per thread
+// the counter block: read back by the host once per round
+enum ImpCounter { IMP_FAILS = 0, IMP_LEFT = 1, IMP_BAD = 2, IMP_TRANSFERS = 3, IMP_COUNTERS = 4 };
+
+ZK_IMP_DEV void imp_min(uint32_t *p, uint32_t v) {
+#ifdef ZK_HOST_EMUL
+    if (v < *p) *p = v;
+#else
+    atomicMin(p, v);
+#endif
+}
+ZK_IMP_DEV void imp_inc(uint32_t *p) {
+#ifdef ZK_HOST_EMUL
+    ++*p;
+#else
+    atomicAdd(p, 1u);
+#endif
+}
+
+// ---- 0. start ----------------------------------------------------------------------------------------------------------
+// kind == NULL: every transaction is a transfer (the confidential block).  A transfer starts undecided and applied; its
+// key_a (the chain key) and key_b must be < n_keys.  An issue or destroy takes fixed[k] as its verdict and is applied iff
+// it is 1; an applied one's key_a must be < n_keys (a failed one touches nothing, whatever its slot).  Any fixed byte is
+// taken as it is, IMP_UNDECIDED included: only a transfer is ever undecided (imp_undecided).  An unknown kind, or an index
+// out of range, puts the lowest such transaction in cnt[IMP_BAD].  fixed and verdict may be the same array.
+ZK_IMP_DEV void imp_start(size_t k, uint32_t n_keys, const uint8_t *kind, const uint32_t *key_a, const uint32_t *key_b,
+                          const uint8_t *fixed, uint8_t *verdict, uint8_t *applied, uint32_t *cnt) {
+    const uint8_t kd = kind ? kind[k] : IMP_TRANSFER;
+    bool bad;
+    if (kd == IMP_TRANSFER) {
+        verdict[k] = IMP_UNDECIDED;
+        applied[k] = 1;
+        imp_inc(cnt + IMP_TRANSFERS);
+        bad = key_a[k] >= n_keys || key_b[k] >= n_keys;
+    } else {
+        const uint8_t v = fixed[k];
+        verdict[k] = v;
+        applied[k] = v == 1;
+        bad = kd > IMP_DESTROY || (v == 1 && key_a[k] >= n_keys);
+    }
+    if (bad) imp_min(cnt + IMP_BAD, (uint32_t)k);
+}
+
+// ---- 2. compaction -----------------------------------------------------------------------------------------------------
+// A transfer's verdict byte holds IMP_UNDECIDED or the verifier's verdict; an issue's or destroy's holds the caller's byte,
+// whatever it is, so the kind decides first.
+ZK_IMP_DEV bool imp_undecided(size_t k, const uint8_t *kind, const uint8_t *verdict) {
+    return (!kind || kind[k] == IMP_TRANSFER) && verdict[k] == IMP_UNDECIDED;
+}
+// flag[k] = 1 for an undecided transfer; zk_bal_prefix_sum turns the flags into each one's row of the round buffers
+ZK_IMP_DEV void imp_flag(size_t k, const uint8_t *kind, const uint8_t *verdict, uint32_t *flag) { flag[k] = imp_undecided(k, kind, verdict); }
+
+// Item i: word w = i % IMP_WORDS of transaction k = i / IMP_WORDS, when k is undecided: words [0, 88) are its verifier
+// row, with bytes [192, 256) taken from balance_sender[k], words [88, 136) its proof.  Word 0 also records k as the row's
+// transaction.  Byte copies: the caller's arrays need no alignment.
+ZK_IMP_DEV void imp_gather(size_t i, const uint8_t *kind, const uint8_t *verdict, const uint32_t *pos, const uint8_t *rows, const uint8_t *proofs,
+                           const uint8_t *balance_sender, uint32_t *idx, uint8_t *round_rows, uint8_t *round_proofs) {
+    const size_t k = i / IMP_WORDS;
+    const uint32_t w = (uint32_t)(i % IMP_WORDS);
+    if (!imp_undecided(k, kind, verdict)) return;
+    const size_t j = pos[k];
+    if (!w) idx[j] = (uint32_t)k;
+    const uint32_t o = 4 * w;
+    const uint8_t *src;
+    uint8_t *dst;
+    if (o < IMP_ROW) {
+        src = o >= IMP_BS && o < IMP_BS + 64 ? balance_sender + 64 * k + (o - IMP_BS) : rows + IMP_ROW * k + o;
+        dst = round_rows + IMP_ROW * j + o;
+    } else {
+        src = proofs + 192 * k + (o - IMP_ROW);
+        dst = round_proofs + 192 * j + (o - IMP_ROW);
+    }
+#pragma unroll
+    for (int b = 0; b < 4; b++) dst[b] = src[b];
+}
+
+// the confidential state pass's tx_points (amount_sender | amount_recipient | fee_sender | randomness) from the rows:
+// item i is word i % 32 of transaction i / 32, slots 2, 3, 5, 4
+ZK_IMP_DEV void imp_tx_points(size_t i, const uint8_t *rows, uint8_t *tx_points) {
+    const size_t k = i >> 5;
+    const uint32_t w = (uint32_t)(i & 31), slot = w >> 3, from = slot < 2 ? 2 + slot : 7 - slot;
+    const uint8_t *src = rows + IMP_ROW * k + 32 * from + 4 * (w & 7);
+    uint8_t *dst = tx_points + 128 * k + 4 * w;
+#pragma unroll
+    for (int b = 0; b < 4; b++) dst[b] = src[b];
+}
+
+// ---- 4. decisions ------------------------------------------------------------------------------------------------------
+// row j of m: transaction idx[j] with verdict rv[j].  A failure lowers its chain's first_fail (IMP_NONE before the pass)
+// and counts in cnt[IMP_FAILS].
+ZK_IMP_DEV void imp_fail(size_t j, const uint32_t *idx, const uint32_t *key_a, const uint8_t *rv, uint32_t *first_fail, uint32_t *cnt) {
+    if (rv[j] == 1) return;
+    const uint32_t k = idx[j];
+    imp_min(first_fail + key_a[k], k);
+    imp_inc(cnt + IMP_FAILS);
+}
+// after every imp_fail: a transaction at or before its chain's first failure takes its verdict, and is applied iff it
+// passed; one after it stays undecided and applied, and counts in cnt[IMP_LEFT]
+ZK_IMP_DEV void imp_decide(size_t j, const uint32_t *idx, const uint32_t *key_a, const uint8_t *rv, const uint32_t *first_fail,
+                           uint8_t *verdict, uint8_t *applied, uint32_t *cnt) {
+    const uint32_t k = idx[j];
+    if (k <= first_fail[key_a[k]]) {
+        verdict[k] = rv[j];
+        applied[k] = rv[j] == 1;
+    } else {
+        imp_inc(cnt + IMP_LEFT);
+    }
+}
+
+}  // namespace zkimp

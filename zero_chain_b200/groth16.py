@@ -1008,6 +1008,59 @@ class DestroyTx:
                                    self.dummy_balance, self.rvk, self.g_epoch, self.nonce)
 
 
+def _asset_slots(name: str, slots: list, balances, pendings, flags, txs, verdicts, next_asset_id: int, new_slot_flags: int):
+    """Asset ids, then slots, once the issue and destroy verdicts are known: the passing issues are numbered from
+    next_asset_id, and every (asset_id, key) a transaction names is resolved to a row of the slot table; new ones are
+    appended to `slots` (in place) and to the table, absent, with new_slot_flags.  A failing issue or destroy names no slot.
+    Returns ((balances, pendings, flags) of the grown table, asset_ids, slot_a, slot_b)."""
+    n = len(txs)
+    index = {s: i for i, s in enumerate(slots)}
+    bal, pend, fl = bytearray(_cat(balances, 64)), bytearray(_cat(pendings, 64)), bytearray(flags)
+
+    def slot(asset_id, key):
+        s = (asset_id, key)
+        if s not in index:
+            index[s] = len(slots)
+            slots.append(s)
+            bal.extend(bytes(64)); pend.extend(bytes(64)); fl.append(new_slot_flags & 0xFF & ~(ACCOUNT_BALANCE | ACCOUNT_PENDING))
+        return index[s]
+    asset_ids = [None] * n
+    next_id = int(next_asset_id)
+    none = 0xFFFFFFFF                                         # past every slot: a failed issue or destroy touches nothing
+    slot_a, slot_b = np.full(n, none, np.uint32), np.full(n, none, np.uint32)
+    for k, t in enumerate(txs):
+        if t.kind == ASSET_ISSUE:
+            if verdicts[k] != 1:
+                continue
+            if next_id > ASSET_ID_MAX:
+                raise ValueError("%s: asset id %d would pass 2^32 - 1" % (name, next_id))
+            asset_ids[k] = next_id
+            slot_a[k] = slot(next_id, t.issuer)
+            next_id += 1
+        elif t.kind == ASSET_DESTROY:
+            if verdicts[k] == 1:
+                slot_a[k] = slot(t.asset_id, t.owner)
+        else:
+            slot_a[k] = slot(t.asset_id, t.address_sender)
+            slot_b[k] = slot(t.asset_id, t.address_recipient)
+    return (bytes(bal), bytes(pend), bytes(fl)), asset_ids, slot_a, slot_b
+
+
+def _asset_events(kinds, ba: bytes, ev: bytes, ef: bytes, st: bytes) -> list:
+    """The event ciphertexts of each applied transaction, from zk_assets_block's outputs (see import_assets_block)."""
+    events = [None] * len(kinds)
+    for k in range(len(kinds)):
+        if st[k] != BLOCK_APPLIED:
+            continue
+        if kinds[k] == ASSET_TRANSFER:
+            events[k] = ba[64 * k:64 * k + 64]
+        elif kinds[k] == ASSET_ISSUE:
+            events[k] = ev[128 * k:128 * k + 64]
+        else:
+            events[k] = tuple(ev[128 * k + 64 * w:128 * k + 64 * w + 64] if ef[k] >> w & 1 else b"" for w in range(2))
+    return events
+
+
 def import_assets_block(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
     """Verify and apply a block of encrypted-asset extrinsics the way the runtime does, one after another.  state =
     (slots, balances, pendings, flags): slots lists the (asset_id, enc_key) of each row of the slot table, the rest as
@@ -1039,38 +1092,9 @@ def import_assets_block(ctx: Context, pvk: PreparedVerifyingKey, state, txs, pro
     if len(fixed):
         pts = b"".join(txs[k].verify_points() for k in fixed.tolist())
         verdicts[fixed] = verify_proofs_with_points(pvk, proof_rows[fixed].tobytes(), pts, CONFIDENTIAL_POINTS)
-    # asset ids, then slots
-    index = {s: i for i, s in enumerate(slots)}
-    bal, pend, fl = bytearray(_cat(balances, 64)), bytearray(_cat(pendings, 64)), bytearray(flags)
-
-    def slot(asset_id, key):
-        s = (asset_id, key)
-        if s not in index:
-            index[s] = len(slots)
-            slots.append(s)
-            bal.extend(bytes(64)); pend.extend(bytes(64)); fl.append(new_slot_flags & 0xFF & ~(ACCOUNT_BALANCE | ACCOUNT_PENDING))
-        return index[s]
-    asset_ids = [None] * n
-    next_id = int(next_asset_id)
-    none = 0xFFFFFFFF                                         # past every slot: a failed issue or destroy touches nothing
-    slot_a, slot_b = np.full(n, none, np.uint32), np.full(n, none, np.uint32)
-    for k, t in enumerate(txs):
-        if t.kind == ASSET_ISSUE:
-            if verdicts[k] != 1:
-                continue
-            if next_id > ASSET_ID_MAX:
-                raise ValueError("import_assets_block: asset id %d would pass 2^32 - 1" % next_id)
-            asset_ids[k] = next_id
-            slot_a[k] = slot(next_id, t.issuer)
-            next_id += 1
-        elif t.kind == ASSET_DESTROY:
-            if verdicts[k] == 1:
-                slot_a[k] = slot(t.asset_id, t.owner)
-        else:
-            slot_a[k] = slot(t.asset_id, t.address_sender)
-            slot_b[k] = slot(t.asset_id, t.address_recipient)
+    table, asset_ids, slot_a, slot_b = _asset_slots("import_assets_block", slots, balances, pendings, flags, txs, verdicts, next_asset_id,
+                                                    new_slot_flags)
     tx_points = b"".join(t.points() for t in txs)
-    table = (bytes(bal), bytes(pend), bytes(fl))
     is_transfer = kinds == ASSET_TRANSFER
     chains = None
     rounds = 0
@@ -1099,18 +1123,126 @@ def import_assets_block(ctx: Context, pvk: PreparedVerifyingKey, state, txs, pro
                 verdicts[k] = got_of[k]
                 if got_of[k] != 1:
                     break
-    events = [None] * n
-    ba, ev, ef, st = out[1], out[2], out[3], out[4]
-    for k in range(n):
-        if st[k] != BLOCK_APPLIED:
-            continue
-        if kinds[k] == ASSET_TRANSFER:
-            events[k] = ba[64 * k:64 * k + 64]
-        elif kinds[k] == ASSET_ISSUE:
-            events[k] = ev[128 * k:128 * k + 64]
-        else:
-            events[k] = tuple(ev[128 * k + 64 * w:128 * k + 64 * w + 64] if ef[k] >> w & 1 else b"" for w in range(2))
+    events = _asset_events(kinds, *out[1:5])
     return [int(v) for v in verdicts], asset_ids, events, (slots,) + out[5:], rounds
+
+
+# ---- block import in one call: the rounds of import_confidential_block / import_assets_block on the device --------------
+def _import_error(name: str, e: ZkError):
+    """zk_import_*'s ZK_ERR_INVALID for an index out of range becomes the drivers' ValueError"""
+    if e.code == -2 and "out of range" in str(e):
+        return ValueError("%s: %s" % (name, e))
+    return e
+
+
+def _confidential_rows(txs) -> bytes:
+    """each transfer's 11 verifier points in confidential_points order, balance_sender (slots 6-7) zero"""
+    return b"".join(t.address_sender + t.address_recipient + t.amount_sender + t.amount_recipient + t.randomness + t.fee_sender +
+                    bytes(64) + t.rvk + t.g_epoch + t.nonce for t in txs)
+
+
+def confidential_import(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, proofs):
+    """import_confidential_block in one call (zk_import_confidential_block): the rounds run on the device, between one
+    upload and one download, and the proofs are checked on ctx.  Same arguments, result and errors, except that a key of
+    another shape raises SynthesisError(MalformedVerifyingKey) even for a block without transfers."""
+    balances, pendings, flags = accounts
+    n_acct, n = len(flags), len(txs)
+    if any(not (0 <= t.sender < 2**32 and 0 <= t.recipient < 2**32) for t in txs):
+        raise ValueError("confidential_import: account index out of range")
+    proofs = _cat(proofs, 192)
+    bal, pend, fl = _cat(balances, 64), _cat(pendings, 64), bytes(flags)
+    assert len(proofs) == 192 * n and len(bal) == len(pend) == 64 * n_acct
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    idx = lambda v: np.array(v or [0], np.uint32)
+    z = lambda m: np.zeros(max(m, 1), np.uint8)
+    v, ba, st, nb, npd, nf = z(n), z(64 * n), z(n), z(64 * n_acct), z(64 * n_acct), z(n_acct)
+    rounds = C.c_uint(0)
+    if pvk.ctx is not ctx:
+        pvk.ctx.sync()
+    try:
+        _ck(_lib.lib().zk_import_confidential_block(ctx._h, pvk._h, n_acct, _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n,
+                                                    _p(idx([t.sender for t in txs])), _p(idx([t.recipient for t in txs])),
+                                                    _p(buf(_confidential_rows(txs))), _p(buf(proofs)), _p(v), _p(ba), _p(st), _p(nb), _p(npd),
+                                                    _p(nf), C.byref(rounds)))
+    except ZkError as e:
+        raise _import_error("confidential_import", e) from None
+    return ([int(x) for x in v[:n]], (nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes()),
+            ba[:64 * n].tobytes(), rounds.value)
+
+
+def confidential_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_accounts: int, d_balances_ptr: int, d_pendings_ptr: int,
+                               d_flags_ptr: int, n_tx: int, d_sender_ptr: int, d_recipient_ptr: int, d_rows_ptr: int, d_proofs_ptr: int,
+                               d_verdicts_ptr: int, d_balance_after_ptr: int, d_status_ptr: int, d_new_balances_ptr: int,
+                               d_new_pendings_ptr: int, d_new_flags_ptr: int) -> int:
+    """zk_import_confidential_block_device on device pointers (d_sender / d_recipient: uint32; d_rows: n_tx * 352 bytes in
+    confidential_points order, slots 6-7 ignored).  Blocks on the context's stream once before the first round and once
+    after each; returns the number of rounds, with the outputs complete."""
+    v = lambda x: C.c_void_p(x) if x else None
+    rounds = C.c_uint(0)
+    _ck(_lib.lib().zk_import_confidential_block_device(ctx._h, pvk._h, n_accounts, v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr),
+                                                       n_tx, v(d_sender_ptr), v(d_recipient_ptr), v(d_rows_ptr), v(d_proofs_ptr),
+                                                       v(d_verdicts_ptr), v(d_balance_after_ptr), v(d_status_ptr), v(d_new_balances_ptr),
+                                                       v(d_new_pendings_ptr), v(d_new_flags_ptr), C.byref(rounds)))
+    return rounds.value
+
+
+def assets_import(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
+    """import_assets_block with the transfer rounds in one call (zk_import_assets_block).  The issue and destroy proofs
+    are verified first, and asset ids and slots resolved from their verdicts, exactly as import_assets_block does; the
+    rounds then run on the device between one upload and one download, with the transfer proofs checked on ctx.  Same
+    arguments, result and errors, except for a key of another shape, as confidential_import."""
+    slots, balances, pendings, flags = state
+    slots = [(int(a), _pt32(k)) for a, k in slots]
+    n = len(txs)
+    proofs = _cat(proofs, 192)
+    assert len(proofs) == 192 * n and len(flags) == len(slots)
+    proof_rows = np.frombuffer(proofs, np.uint8).reshape(n, 192) if n else np.zeros((0, 192), np.uint8)
+    kinds = np.array([t.kind for t in txs], np.uint8)
+    fixed_v = np.zeros(n, np.uint8)
+    fixed = np.flatnonzero(kinds != ASSET_TRANSFER)
+    if len(fixed):
+        pts = b"".join(txs[k].verify_points() for k in fixed.tolist())
+        fixed_v[fixed] = verify_proofs_with_points(pvk, proof_rows[fixed].tobytes(), pts, CONFIDENTIAL_POINTS)
+    (bal, pend, fl), asset_ids, slot_a, slot_b = _asset_slots("assets_import", slots, balances, pendings, flags, txs, fixed_v,
+                                                              next_asset_id, new_slot_flags)
+    n_slots = len(fl)
+    rows = b"".join(t.verify_points(bytes(64)) if t.kind == ASSET_TRANSFER else bytes(32 * CONFIDENTIAL_POINTS) for t in txs)
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    idx = lambda a: a if n else np.zeros(1, np.uint32)
+    z = lambda m: np.zeros(max(m, 1), np.uint8)
+    v, ba, ev, ef, st = z(n), z(64 * n), z(128 * n), z(n), z(n)
+    nb, npd, nf = z(64 * n_slots), z(64 * n_slots), z(n_slots)
+    rounds = C.c_uint(0)
+    if pvk.ctx is not ctx:
+        pvk.ctx.sync()
+    try:
+        _ck(_lib.lib().zk_import_assets_block(ctx._h, pvk._h, n_slots, _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n, _p(buf(kinds.tobytes())),
+                                              _p(idx(slot_a)), _p(idx(slot_b)), _p(buf(b"".join(t.points() for t in txs))), _p(buf(rows)),
+                                              _p(buf(proofs)), _p(buf(fixed_v.tobytes())), _p(v), _p(ba), _p(ev), _p(ef), _p(st), _p(nb),
+                                              _p(npd), _p(nf), C.byref(rounds)))
+    except ZkError as e:
+        raise _import_error("assets_import", e) from None
+    events = _asset_events(kinds, ba[:64 * n].tobytes(), ev[:128 * n].tobytes(), ef[:n].tobytes(), st[:n].tobytes())
+    table = (nb[:64 * n_slots].tobytes(), npd[:64 * n_slots].tobytes(), nf[:n_slots].tobytes())
+    return [int(x) for x in v[:n]], asset_ids, events, (slots,) + table, rounds.value
+
+
+def assets_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: int, d_balances_ptr: int, d_pendings_ptr: int, d_flags_ptr: int,
+                         n_tx: int, d_kind_ptr: int, d_slot_a_ptr: int, d_slot_b_ptr: int, d_tx_points_ptr: int, d_rows_ptr: int,
+                         d_proofs_ptr: int, d_fixed_verdicts_ptr: int, d_verdicts_ptr: int, d_balance_after_ptr: int, d_event_ct_ptr: int,
+                         d_event_flags_ptr: int, d_status_ptr: int, d_new_balances_ptr: int, d_new_pendings_ptr: int,
+                         d_new_flags_ptr: int) -> int:
+    """zk_import_assets_block_device on device pointers (slots as assets_block_device; d_rows as confidential_import_device,
+    read at transfers; d_fixed_verdicts: the issue and destroy verdicts).  Blocks as confidential_import_device; returns the
+    number of rounds, with the outputs complete."""
+    v = lambda x: C.c_void_p(x) if x else None
+    rounds = C.c_uint(0)
+    _ck(_lib.lib().zk_import_assets_block_device(ctx._h, pvk._h, n_slots, v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr), n_tx,
+                                                 v(d_kind_ptr), v(d_slot_a_ptr), v(d_slot_b_ptr), v(d_tx_points_ptr), v(d_rows_ptr),
+                                                 v(d_proofs_ptr), v(d_fixed_verdicts_ptr), v(d_verdicts_ptr), v(d_balance_after_ptr),
+                                                 v(d_event_ct_ptr), v(d_event_flags_ptr), v(d_status_ptr), v(d_new_balances_ptr),
+                                                 v(d_new_pendings_ptr), v(d_new_flags_ptr), C.byref(rounds)))
+    return rounds.value
 
 
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
