@@ -522,6 +522,44 @@ int zk_import_assets_block_device(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots
                                   const uint8_t *d_fixed_verdicts, uint8_t *d_verdicts, uint8_t *d_balance_after, uint8_t *d_event_ct,
                                   uint8_t *d_event_flags, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
                                   uint8_t *d_new_flags, unsigned *rounds);
+/* ---- block import: the proofs and the state of anonymous-balances calls in one call -------------------------------------
+ * zk_import_anonymous_block: anonymous_transfer and issue in block order, verified and applied.  No rounds: an issue's
+ * proof reads only its own fields, and a transfer changes pending balances only, so nothing a proof is checked against
+ * depends on a transfer's verdict.  The call verifies the issues (zk_groth16_verify_points_batch with conf_pvk, 11
+ * points), runs the state pass (zk_anonymous_calls_block) with the issue verdicts as the mask and no transfer applied,
+ * verifies the transfers on the 52 points that pass gives (anon_pvk), and runs the state pass again with all the verdicts.
+ * A block without issues takes zk_balances_anonymous_block's passes; a block without transfers ends after the first pass.
+ *
+ * The arguments of zk_anonymous_calls_block, with the verifier's inputs in place of applied:
+ * kind: as zk_anonymous_calls_block (0 transfer, 1 issue); NULL: every transaction is a transfer.
+ * tx_extra[k]: rvk | nonce, read for issues too.
+ * issue_fields: n_tx * 96 B, an issue's fee | balance; read at issues only, may be NULL when the block has no issue.
+ * proofs: n_tx * 192 B.  anon_pvk: a prepared key of 52-point proofs; conf_pvk: one of 11-point proofs, or NULL when the
+ *   block has no issue.  Both on the context's device, ready to use.
+ * verdicts[k]: as zk_groth16_verify_points_batch gives it (1 passes).  An issue's from conf_pvk on (issuer, issuer, total,
+ *   total, randomness, fee, balance, rvk, g_epoch, nonce), with issuer = keys[members[12 k]], total and randomness slots 0
+ *   and 12 of its tx_points row; a transfer's from anon_pvk on its 52 verify_points of the first state pass.
+ * enc_balances, issued, tx_status, new_balances, new_pendings, new_flags: zk_anonymous_calls_block's outputs for the final
+ *   verdicts; issued is zero bytes where nothing is written.
+ * ZK_ERR_INVALID, naming the lowest such transaction in zk_last_error, for an unknown kind, a transfer's member >=
+ *   n_accounts, an issuer >= n_accounts (an issue's other 11 member entries are ignored), or an issue when conf_pvk or
+ *   issue_fields is NULL; and as zk_anonymous_calls_block for NULL arguments (kind excepted) and sizes.
+ *   ZK_ERR_MALFORMED_VK for an anon_pvk of other than 52 points or a conf_pvk of other than 11.  ZK_ERR_DECODE as
+ *   zk_anonymous_calls_block; the outputs are then undefined. */
+int zk_import_anonymous_block(zk_ctx *ctx, const zk_pvk *anon_pvk, const zk_pvk *conf_pvk, size_t n_accounts, const uint8_t *keys,
+                              const uint8_t *balances, const uint8_t *pendings, const uint8_t *acct_flags, size_t n_tx, const uint8_t *kind,
+                              const uint32_t *members, const uint8_t *tx_points, const uint8_t *tx_extra, const uint8_t *issue_fields,
+                              const uint8_t *g_epoch, const uint8_t *proofs, uint8_t *verdicts, uint8_t *enc_balances, uint8_t *issued,
+                              uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags);
+/* the same with device pointers (d_members 4-byte aligned).  The call blocks on the context's stream once, to read the
+ * number of issues and of transfers and the lowest bad transaction, and returns with the outputs complete; it reports
+ * ZK_ERR_DECODE itself. */
+int zk_import_anonymous_block_device(zk_ctx *ctx, const zk_pvk *anon_pvk, const zk_pvk *conf_pvk, size_t n_accounts, const uint8_t *d_keys,
+                                     const uint8_t *d_balances, const uint8_t *d_pendings, const uint8_t *d_acct_flags, size_t n_tx,
+                                     const uint8_t *d_kind, const uint32_t *d_members, const uint8_t *d_tx_points, const uint8_t *d_tx_extra,
+                                     const uint8_t *d_issue_fields, const uint8_t *d_g_epoch, const uint8_t *d_proofs, uint8_t *d_verdicts,
+                                     uint8_t *d_enc_balances, uint8_t *d_issued, uint8_t *d_tx_status, uint8_t *d_new_balances,
+                                     uint8_t *d_new_pendings, uint8_t *d_new_flags);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

@@ -10,6 +10,12 @@
                one upload, the rounds on the device, one download; assets_import verifies the issues and destroys first)
       verify   verify_proofs_with_points_device alone on every proof of the block, on device-resident points
   - the rounds, and the ratios call / verify and driver / verify.
+  - for a block of --anon-tx anonymous-balances calls (transfers, with --issue-frac issues) over --accounts accounts, the
+    same three arms: the driver import_anonymous_calls_block (torch index ops between the launches), the one C call
+    anonymous_import (zk_import_anonymous_block), and the two verify_proofs_with_points_device launches alone (issues on
+    11 points, transfers on 52) on device-resident rows.  Proofs are forged from toy keys of the real shapes' input counts
+    (tests/import_anon_corpus.py); the outputs are checked against anon_issue_coracle.c.
+A leg with 0 transactions is skipped.
 --fail-rate is the fraction of transfers (and of issues and destroys) whose proof fails; a transfer after a failure in its
 chain is proven against the balance without it, so each failure costs a round.  Proofs are forged from a toy key's
 trapdoor (tests/import_corpus.py, 22 public inputs: the verifier does the work of the real key per proof).  Every output
@@ -28,6 +34,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tests import import_anon_corpus as iac               # noqa: E402
 from tests import import_corpus as ic                     # noqa: E402
 from zero_chain_b200 import groth16 as zk                  # noqa: E402
 
@@ -59,6 +66,7 @@ def main():
     ap.add_argument("--conf-tx", type=int, default=8192)
     ap.add_argument("--accounts", type=int, default=1024)
     ap.add_argument("--asset-tx", type=int, default=4096)
+    ap.add_argument("--anon-tx", type=int, default=4096)
     ap.add_argument("--slots", type=int, default=1024)
     ap.add_argument("--issue-frac", type=float, default=0.05)
     ap.add_argument("--destroy-frac", type=float, default=0.02)
@@ -104,7 +112,19 @@ def main():
         return {"ms": {k: round(v, 3) for k, v in med.items()}, "call_over_verify": round(med["call"] / med["verify"], 3),
                 "driver_over_verify": round(med["driver"] / med["verify"], 3)}
 
-    # ---- confidential transfers
+    if a.conf_tx:
+        res["confidential"] = confidential_leg(a, ctx, key, pvk, measure, verify_alone)
+    if a.asset_tx:
+        res["assets"] = assets_leg(a, ctx, key, pvk, measure, verify_alone)
+    if a.anon_tx:
+        res["anonymous"] = anonymous_leg(a, ctx, measure)
+    res["outputs_equal_oracle"] = True
+    pvk.free()
+    ctx.close()
+    print(json.dumps(res))
+
+
+def confidential_leg(a, ctx, key, pvk, measure, verify_alone):
     log("confidential corpus: %d transfers over %d accounts" % (a.conf_tx, a.accounts))
     blk = ic.confidential(key, a.accounts, a.conf_tx, a.seed, fail_frac=a.fail_rate, skew=a.skew,
                           state_call=lambda *x: zk.confidential_block(ctx, *x))
@@ -120,12 +140,13 @@ def main():
             assert out == v_want, "verification alone differs"
         else:
             assert out == want, "%s differs" % k
-    res["confidential"] = dict(measure("confidential", lambda: zk.import_confidential_block(ctx, pvk, blk.accounts, blk.txs, blk.proofs),
+    return dict(measure("confidential", lambda: zk.import_confidential_block(ctx, pvk, blk.accounts, blk.txs, blk.proofs),
                                        lambda: zk.confidential_import(ctx, pvk, blk.accounts, blk.txs, blk.proofs),
                                        verify_alone(blk.rows, blk.proofs), check_conf),
-                               n_tx=a.conf_tx, accounts=a.accounts, rounds=want[3], failures=sum(v != 1 for v in want[0]))
+                n_tx=a.conf_tx, accounts=a.accounts, rounds=want[3], failures=sum(v != 1 for v in want[0]))
 
-    # ---- encrypted-asset calls
+
+def assets_leg(a, ctx, key, pvk, measure, verify_alone):
     log("asset corpus: %d calls over %d slots" % (a.asset_tx, a.slots))
     ab = ic.assets(key, a.slots, a.asset_tx, a.seed + 1, fail_frac=a.fail_rate, fixed_fail_frac=a.fail_rate, issue_frac=a.issue_frac,
                    destroy_frac=a.destroy_frac, skew=a.skew, state_call=lambda *x: zk.assets_block(ctx, *x))
@@ -142,13 +163,52 @@ def main():
             assert out == av_want, "verification alone differs"
         else:
             assert out == awant, "%s differs" % k
-    res["assets"] = dict(measure("assets", lambda: zk.import_assets_block(ctx, pvk, *ab.args()), lambda: zk.assets_import(ctx, pvk, *ab.args()),
+    return dict(measure("assets", lambda: zk.import_assets_block(ctx, pvk, *ab.args()), lambda: zk.assets_import(ctx, pvk, *ab.args()),
                                  verify_alone(ab.rows, ab.proofs), check_assets),
-                         n_tx=a.asset_tx, slots=a.slots, rounds=awant[4], failures=sum(v != 1 for v in awant[0]))
-    res["outputs_equal_oracle"] = True
-    pvk.free()
-    ctx.close()
-    print(json.dumps(res))
+                n_tx=a.asset_tx, slots=a.slots, rounds=awant[4], failures=sum(v != 1 for v in awant[0]))
+
+
+def anonymous_leg(a, ctx, measure):
+    import torch
+    anon, conf = iac.ForgeKey(zk.ANONYMOUS_POINTS, 71), iac.ForgeKey(zk.CONFIDENTIAL_POINTS, 171)
+    apvk, cpvk = zk.PreparedVerifyingKey.prepare(ctx, anon.params_bytes), zk.PreparedVerifyingKey.prepare(ctx, conf.params_bytes)
+    log("anonymous corpus: %d calls over %d accounts" % (a.anon_tx, a.accounts))
+    blk = iac.block(anon, conf, a.accounts, a.anon_tx, a.seed + 2, issue_frac=a.issue_frac, fail_frac=a.fail_rate, skew=a.skew)
+    want = zk.anonymous_import(ctx, apvk, cpvk, *blk.args())
+    log("C oracle (anonymous)")
+    o = blk.oracle(want[0])
+    assert want[0] == blk.intended, "anonymous verdicts differ from the intended ones"
+    assert want[2] == o[0] and want[1] == o[4:], "the anonymous import differs from the C oracle"
+    assert all(x == (o[2][64 * k:64 * k + 64] if x is not None else None) for k, x in enumerate(want[3])), "issued differs from the C oracle"
+    iss = [k for k, t in enumerate(blk.txs) if t.kind == zk.ANON_ISSUE]
+    tr = [k for k, t in enumerate(blk.txs) if t.kind == zk.ANON_TRANSFER]
+    # the verifier's rows, device-resident: the issues' 11 points, the transfers' 52 from the state the oracle gives
+    dev = torch.device("cuda", 0)
+    up = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev) if b else torch.zeros(1, dtype=torch.uint8, device=dev)
+    d_iss = up(b"".join(blk.txs[k].verify_points(blk.accounts[0], blk.g_epoch) for k in iss))
+    d_tr = up(b"".join(o[1][1664 * k:1664 * k + 1664] for k in tr))
+    d_ip, d_tp = up(b"".join(blk.proofs[k] for k in iss)), up(b"".join(blk.proofs[k] for k in tr))
+    d_out = torch.zeros(len(blk.txs) + 1, dtype=torch.uint8, device=dev)
+    v_want = bytes(blk.intended[k] for k in iss + tr)
+    torch.cuda.synchronize()
+
+    def verify():
+        if iss:
+            zk.verify_proofs_with_points_device(cpvk, len(iss), d_ip.data_ptr(), d_iss.data_ptr(), zk.CONFIDENTIAL_POINTS, d_out.data_ptr())
+        if tr:
+            zk.verify_proofs_with_points_device(apvk, len(tr), d_tp.data_ptr(), d_tr.data_ptr(), zk.ANONYMOUS_POINTS,
+                                                d_out.data_ptr() + len(iss))
+        ctx.sync()
+        return d_out[:len(blk.txs)].cpu().numpy().tobytes()
+
+    def check(k, out):
+        assert out == (v_want if k == "verify" else want), "%s differs" % k
+    r = dict(measure("anonymous", lambda: zk.import_anonymous_calls_block(ctx, apvk, cpvk, *blk.args()),
+                     lambda: zk.anonymous_import(ctx, apvk, cpvk, *blk.args()), verify, check),
+             n_tx=a.anon_tx, accounts=a.accounts, issues=len(iss), failures=sum(v != 1 for v in want[0]))
+    apvk.free()
+    cpvk.free()
+    return r
 
 
 if __name__ == "__main__":

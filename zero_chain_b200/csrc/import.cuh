@@ -13,8 +13,18 @@
 // undecided transfer as passed, and its state pass is the final state; a round that leaves nothing undecided is followed
 // by one last state pass.  Issues and destroys (zk_import_assets_block) carry the caller's verdicts from the start.
 //
+// zk_import_anonymous_block needs no rounds: an issue's proof reads only its own fields, and a transfer changes pending
+// balances only, so nothing a proof is checked against depends on a transfer's verdict.  Its passes (section 5) are
+//   1. imp_an_start: check each transaction's kind and indices, count issues and transfers, flag the issues;
+//      zk_bal_prefix_sum turns the flags into each issue's compact row (a transfer's row is k - the issues before k),
+//   2. imp_an_issue_row: each issue's 11 confidential points and its proof, verified with the confidential key,
+//   3. imp_an_scatter: the issue verdicts into verdicts (transfers 0: not applied), then the state pass
+//      (zk_anonymous_calls_block) with verdicts as the mask,
+//   4. imp_an_gather: each transfer's 52 points from that pass and its proof, verified with the anonymous key,
+//   5. imp_an_scatter: the transfer verdicts, then the state pass again.
+//
 // Plain integer code, one function per item and thread of each pass; the same source compiles with ZK_HOST_EMUL for the
-// CPU test (tests/host_emul/emul_import.cpp), which runs the rounds as loops over the items.
+// CPU tests (tests/host_emul/emul_import.cpp, emul_import_anon.cpp), which run the passes as loops over the items.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -142,6 +152,101 @@ ZK_IMP_DEV void imp_decide(size_t j, const uint32_t *idx, const uint32_t *key_a,
     } else {
         imp_inc(cnt + IMP_LEFT);
     }
+}
+
+// ---- 5. zk_import_anonymous_block --------------------------------------------------------------------------------------
+constexpr uint8_t IMP_AN_TRANSFER = 0, IMP_AN_ISSUE = 1;        // zk_anonymous_calls_block's kinds
+constexpr int IMP_AN_RING = 12;
+constexpr int IMP_AN_TX_POINTS = IMP_AN_RING + 1;               // left ciphertexts | right ciphertext
+constexpr int IMP_AN_ROW = 32 * (4 * IMP_AN_RING + 4);          // bytes of a transfer's verifier row (52 points)
+constexpr int IMP_AN_ISSUE_WORDS = (IMP_ROW + 192) / 4;         // an issue's row and proof, one 4-byte word per thread
+constexpr int IMP_AN_WORDS = (IMP_AN_ROW + 192) / 4;            // a transfer's
+constexpr int IMP_ISSUES = IMP_FAILS;                           // the counter block: issues in the slot the rounds count failures in
+
+// kind == NULL: every transaction is a transfer.  A transfer's 12 members must be < n_acct; an issue's issuer (members[12 k])
+// must be, and the block must have what an issue's verification reads (issues_ok: a confidential key and issue_fields).
+// Any other kind is bad.  The lowest bad transaction goes to cnt[IMP_BAD]; flag[k] = 1 for an issue.
+ZK_IMP_DEV void imp_an_start(size_t k, uint32_t n_acct, bool issues_ok, const uint8_t *kind, const uint32_t *members, uint32_t *flag,
+                             uint32_t *cnt) {
+    const uint8_t kd = kind ? kind[k] : IMP_AN_TRANSFER;
+    const uint32_t *m = members + IMP_AN_RING * k;
+    bool bad = false;
+    if (kd == IMP_AN_TRANSFER) {
+        for (int i = 0; i < IMP_AN_RING; i++) bad |= m[i] >= n_acct;
+        imp_inc(cnt + IMP_TRANSFERS);
+    } else if (kd == IMP_AN_ISSUE) {
+        bad = !issues_ok || m[0] >= n_acct;
+        imp_inc(cnt + IMP_ISSUES);
+    } else {
+        bad = true;
+    }
+    flag[k] = kd == IMP_AN_ISSUE;
+    if (bad) imp_min(cnt + IMP_BAD, (uint32_t)k);
+}
+
+// Item i: word w = i % IMP_AN_ISSUE_WORDS of transaction k = i / IMP_AN_ISSUE_WORDS, when k is an issue; pos[k] is its row.
+// Words [0, 88) are verify_confidential_proof's 11 points over (issuer, issuer, total, total, randomness, fee, balance, rvk,
+// g_epoch, nonce): keys[issuer], tx_points slots 0 and 12, issue_fields (fee | balance), tx_extra (rvk | nonce) and g_epoch.
+// Words [88, 136) are its proof.  Byte copies: the caller's arrays need no alignment.
+ZK_IMP_DEV void imp_an_issue_row(size_t i, const uint8_t *kind, const uint32_t *pos, const uint8_t *keys, const uint32_t *members,
+                                 const uint8_t *tx_points, const uint8_t *issue_fields, const uint8_t *tx_extra, const uint8_t *g_epoch,
+                                 const uint8_t *proofs, uint8_t *rows, uint8_t *round_proofs) {
+    const size_t k = i / IMP_AN_ISSUE_WORDS;
+    const uint32_t o = 4 * (uint32_t)(i % IMP_AN_ISSUE_WORDS);
+    if (kind[k] != IMP_AN_ISSUE) return;
+    const size_t j = pos[k];
+    const uint8_t *src;
+    uint8_t *dst;
+    if (o < IMP_ROW) {
+        const uint32_t slot = o / 32, b = o % 32;
+        const uint8_t *tp = tx_points + 32 * IMP_AN_TX_POINTS * k;
+        switch (slot) {
+        case 0: case 1: src = keys + 32 * (size_t)members[IMP_AN_RING * k] + b; break;    // address_sender, address_recipient
+        case 2: case 3: src = tp + b; break;                                               // total, twice
+        case 4: src = tp + 32 * IMP_AN_RING + b; break;                                    // randomness
+        case 5: case 6: case 7: src = issue_fields + 96 * k + (o - 32 * 5); break;         // fee, balance
+        case 8: src = tx_extra + 64 * k + b; break;                                        // rvk
+        case 9: src = g_epoch + b; break;
+        default: src = tx_extra + 64 * k + 32 + b; break;                                  // nonce
+        }
+        dst = rows + IMP_ROW * j + o;
+    } else {
+        src = proofs + 192 * k + (o - IMP_ROW);
+        dst = round_proofs + 192 * j + (o - IMP_ROW);
+    }
+#pragma unroll
+    for (int b = 0; b < 4; b++) dst[b] = src[b];
+}
+
+// issues: verdicts[k] = rv[pos[k]] at an issue and 0 at a transfer (not applied in the first state pass); otherwise
+// verdicts[k] = rv[k - pos[k]] at a transfer, issues unchanged.
+ZK_IMP_DEV void imp_an_scatter(size_t k, bool issues, const uint8_t *kind, const uint32_t *pos, const uint8_t *rv, uint8_t *verdicts) {
+    const bool issue = kind[k] == IMP_AN_ISSUE;
+    if (issues)
+        verdicts[k] = issue ? rv[pos[k]] : 0;
+    else if (!issue)
+        verdicts[k] = rv[k - pos[k]];
+}
+
+// Item i: word w = i % IMP_AN_WORDS of transaction k = i / IMP_AN_WORDS, when k is a transfer: words [0, 416) are its 52
+// points from the state pass's verify_points, words [416, 464) its proof, into row k - pos[k].
+ZK_IMP_DEV void imp_an_gather(size_t i, const uint8_t *kind, const uint32_t *pos, const uint8_t *verify_points, const uint8_t *proofs,
+                              uint8_t *rows, uint8_t *round_proofs) {
+    const size_t k = i / IMP_AN_WORDS;
+    const uint32_t o = 4 * (uint32_t)(i % IMP_AN_WORDS);
+    if (kind[k] != IMP_AN_TRANSFER) return;
+    const size_t j = k - pos[k];
+    const uint8_t *src;
+    uint8_t *dst;
+    if (o < IMP_AN_ROW) {
+        src = verify_points + IMP_AN_ROW * k + o;
+        dst = rows + IMP_AN_ROW * j + o;
+    } else {
+        src = proofs + 192 * k + (o - IMP_AN_ROW);
+        dst = round_proofs + 192 * j + (o - IMP_AN_ROW);
+    }
+#pragma unroll
+    for (int b = 0; b < 4; b++) dst[b] = src[b];
 }
 
 }  // namespace zkimp

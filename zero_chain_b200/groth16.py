@@ -1245,6 +1245,59 @@ def assets_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: int, 
     return rounds.value
 
 
+def anonymous_import(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
+    """import_anonymous_calls_block in one call (zk_import_anonymous_block): the issue rows, both verifications, the verdict
+    scatters and both state passes run on the device between one upload and one download, with the proofs checked on
+    ctx.  Same arguments, result and errors (conf_pvk may be None when the block has no issue), except that a key of
+    another shape raises SynthesisError(MalformedVerifyingKey) even when the block does not use it."""
+    keys, balances, pendings, flags = accounts
+    n_acct, n = len(flags), len(txs)
+    if any(not all(0 <= m < 2**32 for m in t.members) for t in txs):
+        raise ValueError("anonymous_import: account index out of range")
+    proofs = _cat(proofs, 192)
+    ky, bal, pend, fl, ge = _cat(keys, 32), _cat(balances, 64), _cat(pendings, 64), bytes(flags), _pt32(g_epoch)
+    assert len(proofs) == 192 * n and len(ky) == 32 * n_acct and len(bal) == len(pend) == 64 * n_acct
+    kind = bytes(t.kind for t in txs)
+    has_issue = ANON_ISSUE in kind
+    fields = b"".join(t.fee + t.balance if t.kind == ANON_ISSUE else bytes(96) for t in txs) if has_issue else b""
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    z = lambda m: np.zeros(max(m, 1), np.uint8)
+    mem = np.array([t.members for t in txs] or [[0]], np.uint32).reshape(-1)
+    v, eb, iss, st = z(n), z(64 * ANONIMITY_SIZE * n), z(64 * n), z(n)
+    nb, npd, nf = z(64 * n_acct), z(64 * n_acct), z(n_acct)
+    for pvk in (anon_pvk, conf_pvk):
+        if pvk is not None and pvk.ctx is not ctx:
+            pvk.ctx.sync()
+    try:
+        _ck(_lib.lib().zk_import_anonymous_block(ctx._h, anon_pvk._h, conf_pvk._h if conf_pvk is not None else None, n_acct, _p(buf(ky)),
+                                                 _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n, _p(buf(kind)), _p(mem),
+                                                 _p(buf(b"".join(t.points() for t in txs))), _p(buf(b"".join(t.rvk + t.nonce for t in txs))),
+                                                 _p(buf(fields)) if has_issue else None, _p(buf(ge)), _p(buf(proofs)), _p(v), _p(eb), _p(iss),
+                                                 _p(st), _p(nb), _p(npd), _p(nf)))
+    except ZkError as e:
+        raise _import_error("anonymous_import", e) from None
+    issued = [iss[64 * k:64 * k + 64].tobytes() if kind[k] == ANON_ISSUE and st[k] == BLOCK_APPLIED else None for k in range(n)]
+    return ([int(x) for x in v[:n]], (nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes()),
+            eb[:64 * ANONIMITY_SIZE * n].tobytes(), issued)
+
+
+def anonymous_import_device(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, n_accounts: int, d_keys_ptr: int,
+                            d_balances_ptr: int, d_pendings_ptr: int, d_flags_ptr: int, n_tx: int, d_kind_ptr: int, d_members_ptr: int,
+                            d_tx_points_ptr: int, d_tx_extra_ptr: int, d_issue_fields_ptr: int, d_g_epoch_ptr: int, d_proofs_ptr: int,
+                            d_verdicts_ptr: int, d_enc_balances_ptr: int, d_issued_ptr: int, d_status_ptr: int, d_new_balances_ptr: int,
+                            d_new_pendings_ptr: int, d_new_flags_ptr: int):
+    """zk_import_anonymous_block_device on device pointers (d_members: uint32; d_kind 0 = every transaction a transfer;
+    d_issue_fields: n_tx * 96 bytes, fee | balance at issues, 0 when the block has none; conf_pvk None likewise).  Blocks on
+    the context's stream once, and returns with the outputs complete."""
+    v = lambda x: C.c_void_p(x) if x else None
+    _ck(_lib.lib().zk_import_anonymous_block_device(ctx._h, anon_pvk._h, conf_pvk._h if conf_pvk is not None else None, n_accounts,
+                                                    v(d_keys_ptr), v(d_balances_ptr), v(d_pendings_ptr), v(d_flags_ptr), n_tx, v(d_kind_ptr),
+                                                    v(d_members_ptr), v(d_tx_points_ptr), v(d_tx_extra_ptr), v(d_issue_fields_ptr),
+                                                    v(d_g_epoch_ptr), v(d_proofs_ptr), v(d_verdicts_ptr), v(d_enc_balances_ptr),
+                                                    v(d_issued_ptr), v(d_status_ptr), v(d_new_balances_ptr), v(d_new_pendings_ptr),
+                                                    v(d_new_flags_ptr)))
+
+
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
     """Engine::pairing for len/96 pairs; 576 bytes each in Fq12::write order."""
     n = len(g1_uncompressed) // 96
