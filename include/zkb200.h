@@ -522,6 +522,50 @@ int zk_import_assets_block_device(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots
                                   const uint8_t *d_fixed_verdicts, uint8_t *d_verdicts, uint8_t *d_balance_after, uint8_t *d_event_ct,
                                   uint8_t *d_event_flags, uint8_t *d_tx_status, uint8_t *d_new_balances, uint8_t *d_new_pendings,
                                   uint8_t *d_new_flags, unsigned *rounds);
+/* zk_import_asset_calls: a block of encrypted-asset calls from the slot table as the module stores it and each transaction
+ *   as its extrinsic carries it.  The call verifies the issues and destroys (zk_groth16_verify_points_batch, 11 points),
+ *   numbers the passing issues, resolves every (AssetId, EncKey) a transaction names to a row of the slot table, appending
+ *   new rows, and runs zk_import_assets_block's rounds on the grown table with those verdicts fixed.
+ * Slot table, n_slots rows: slot_ids (uint32 AssetId), slot_keys (32 B EncKey); balances, pendings, slot_flags as
+ *   zk_assets_block.  (slot_ids[r], slot_keys[r]) must be distinct across rows.
+ * next_asset_id: NextAssetId before the block.  new_slot_flags: the flags of a row the block creates, less bits 0-1
+ *   (ACCOUNT_DUE when current_epoch > 0).
+ * kind[k]: 0 transfer, 1 issue, 2 destroy.  asset_id[k]: read at transfers and destroys, ignored at issues.
+ * rows: n_tx * 11 * 32 B in zk_import_confidential_block's order, the only source of a transaction's fields: slot 0 is the
+ *   sender, issuer or owner; slot 1 the recipient (read at transfers); an issue's total and randomness are slots 2 and 4.
+ *   Slots 6-7 are ignored at transfers (the rounds fill them from the state) and read at issues and destroys (balance /
+ *   dummy_balance).  proofs: n_tx * 192 B.  pvk: the 11-point key of all three kinds, on the context's device, ready to use.
+ * A passing issue (verdict 1) gets the id next_asset_id + (the passing issues before it) and references (its id, issuer); a
+ *   passing destroy references (asset_id, owner); a transfer (asset_id, sender) and (asset_id, recipient).  A failing issue
+ *   or destroy references nothing and consumes no id.  A key in the table maps to its row; a new key gets row n_slots + (the
+ *   new keys whose first reference comes earlier, in block order, sender before recipient), zero ciphertexts and flags
+ *   new_slot_flags & ~3.
+ * Outputs: verdicts, balance_after, event_ct, event_flags, tx_status, new_balances, new_pendings, new_flags as
+ *   zk_import_assets_block, on the grown table; asset_ids[k]: the id of passing issue k, 0 elsewhere; new_slot_ids /
+ *   new_slot_keys: the grown table's (id, key) per row, the first n_slots rows copied; *n_slots_out: its rows.  The table
+ *   outputs need room for n_slots + 2 * n_tx rows.  rounds: as zk_import_assets_block (may be NULL).
+ * ZK_ERR_INVALID, naming the lowest such transaction or row in zk_last_error, for an unknown kind, a passing issue whose id
+ *   would pass 2^32 - 1, a table row whose (id, key) equals an earlier row's, and more than 2^22 rows after the block; for
+ *   NULL arguments (n_slots_out always, the table's when n_slots > 0, the transactions' when n_tx > 0, the table outputs
+ *   when either is) and sizes as zk_assets_block.  ZK_ERR_MALFORMED_VK for a key of other than 11 points.  ZK_ERR_DECODE
+ *   as zk_assets_block; the outputs are then undefined. */
+int zk_import_asset_calls(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const uint32_t *slot_ids, const uint8_t *slot_keys,
+                          const uint8_t *balances, const uint8_t *pendings, const uint8_t *slot_flags, uint32_t next_asset_id,
+                          uint8_t new_slot_flags, size_t n_tx, const uint8_t *kind, const uint32_t *asset_id, const uint8_t *rows,
+                          const uint8_t *proofs, uint8_t *verdicts, uint32_t *asset_ids, uint8_t *balance_after, uint8_t *event_ct,
+                          uint8_t *event_flags, uint8_t *tx_status, uint32_t *new_slot_ids, uint8_t *new_slot_keys, uint8_t *new_balances,
+                          uint8_t *new_pendings, uint8_t *new_flags, size_t *n_slots_out, unsigned *rounds);
+/* the same with device pointers (the uint32 arrays 4-byte aligned; n_slots_out and rounds are host pointers).  The call
+ * blocks on the context's stream twice before the rounds, to read a block of counters: after checking the kinds and the
+ * table (the number of issues and destroys sizes their verification), and after resolving the slots (the new rows, an id
+ * overflow); then as zk_import_assets_block_device.  It returns with the outputs complete. */
+int zk_import_asset_calls_device(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const uint32_t *d_slot_ids, const uint8_t *d_slot_keys,
+                                 const uint8_t *d_balances, const uint8_t *d_pendings, const uint8_t *d_slot_flags, uint32_t next_asset_id,
+                                 uint8_t new_slot_flags, size_t n_tx, const uint8_t *d_kind, const uint32_t *d_asset_id, const uint8_t *d_rows,
+                                 const uint8_t *d_proofs, uint8_t *d_verdicts, uint32_t *d_asset_ids, uint8_t *d_balance_after,
+                                 uint8_t *d_event_ct, uint8_t *d_event_flags, uint8_t *d_tx_status, uint32_t *d_new_slot_ids,
+                                 uint8_t *d_new_slot_keys, uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags,
+                                 size_t *n_slots_out, unsigned *rounds);
 /* ---- block import: the proofs and the state of anonymous-balances calls in one call -------------------------------------
  * zk_import_anonymous_block: anonymous_transfer and issue in block order, verified and applied.  No rounds: an issue's
  * proof reads only its own fields, and a transfer changes pending balances only, so nothing a proof is checked against

@@ -10,6 +10,14 @@
                one upload, the rounds on the device, one download; assets_import verifies the issues and destroys first)
       verify   verify_proofs_with_points_device alone on every proof of the block, on device-resident points
   - the rounds, and the ratios call / verify and driver / verify.
+  - in the asset leg, a fourth arm alternated with the other three:
+      calls    asset_calls_import (zk_import_asset_calls: the issue / destroy verification, the asset numbering and the
+               slot resolution on the device too, from the slot table and the extrinsic fields)
+      calls_c  zk_import_asset_calls alone, on host arrays built once before the reps: what a node calling the C ABI on
+               the fields it already holds pays (asset_calls_import also joins each transaction's verifier row in Python)
+    and the host-clock split of assets_import's host work, each part restated from it and timed in the same reps: the
+    issue / destroy batch (their rows joined, verify_proofs_with_points from host buffers), _asset_slots, and the joins of
+    the transfer rows and tx_points.
   - for a block of --anon-tx anonymous-balances calls (transfers, with --issue-frac issues) over --accounts accounts, the
     same three arms: the driver import_anonymous_calls_block (torch index ops between the launches), the one C call
     anonymous_import (zk_import_anonymous_block), and the two verify_proofs_with_points_device launches alone (issues on
@@ -98,19 +106,22 @@ def main():
             return d_out.cpu().numpy().tobytes()
         return run
 
-    def measure(label, driver, call, verify, check):
-        for fn in (driver, call, verify):            # warm-up: module loads, workspace growth
+    def measure(label, driver, call, verify, check, extra=()):
+        """the arms driver, call, verify and any (name, fn) in extra, alternated; name_over_verify for every arm"""
+        arms = [("driver", driver), ("call", call), ("verify", verify)] + list(extra)
+        for _, fn in arms:                           # warm-up: module loads, workspace growth
             fn()
-        times = {"driver": [], "call": [], "verify": []}
+        times = {k: [] for k, _ in arms}
         for r in range(a.reps):
-            for k, fn in (("driver", driver), ("call", call), ("verify", verify)):
+            for k, fn in arms:
                 ms, out = timed(fn)
                 times[k].append(ms)
                 check(k, out)
             log(label, "rep", r, {k: round(v[-1], 2) for k, v in times.items()})
         med = {k: float(np.median(v)) for k, v in times.items()}
-        return {"ms": {k: round(v, 3) for k, v in med.items()}, "call_over_verify": round(med["call"] / med["verify"], 3),
-                "driver_over_verify": round(med["driver"] / med["verify"], 3)}
+        res = {"ms": {k: round(v, 3) for k, v in med.items()}}
+        res.update({"%s_over_verify" % k: round(med[k] / med["verify"], 3) for k, _ in arms if k != "verify"})
+        return res
 
     if a.conf_tx:
         res["confidential"] = confidential_leg(a, ctx, key, pvk, measure, verify_alone)
@@ -158,14 +169,71 @@ def assets_leg(a, ctx, key, pvk, measure, verify_alone):
     assert all(awant[2][k] == ao[1][64 * k:64 * k + 64] for k, t in enumerate(ab.txs) if t.kind == zk.ASSET_TRANSFER and ao[4][k] == 0)
     av_want = bytes(awant[0])
 
+    split = {"fixed_batch": [], "asset_slots": [], "row_joins": []}
+
+    def host_split():
+        """assets_import's host steps, as it runs them, each on the host clock; returns what it computed"""
+        slots = [(int(x), zk._pt32(k)) for x, k in ab.state[0]]
+        proofs = zk._cat(ab.proofs, 192)
+        t0 = time.perf_counter()
+        n = len(ab.txs)
+        proof_rows = np.frombuffer(proofs, np.uint8).reshape(n, 192)
+        kinds = np.array([t.kind for t in ab.txs], np.uint8)
+        fixed_v = np.zeros(n, np.uint8)
+        fixed = np.flatnonzero(kinds != zk.ASSET_TRANSFER)
+        if len(fixed):
+            pts = b"".join(ab.txs[k].verify_points() for k in fixed.tolist())
+            fixed_v[fixed] = zk.verify_proofs_with_points(pvk, proof_rows[fixed].tobytes(), pts, zk.CONFIDENTIAL_POINTS)
+        t1 = time.perf_counter()
+        table = zk._asset_slots("import_bench", slots, *ab.state[1:], ab.txs, fixed_v, ab.next_asset_id, ab.new_slot_flags)
+        t2 = time.perf_counter()
+        rows = b"".join(t.verify_points(bytes(64)) if t.kind == zk.ASSET_TRANSFER else bytes(32 * zk.CONFIDENTIAL_POINTS) for t in ab.txs)
+        tp = b"".join(t.points() for t in ab.txs)
+        t3 = time.perf_counter()
+        for k, (u, v) in zip(split, ((t0, t1), (t1, t2), (t2, t3))):
+            split[k].append((v - u) * 1e3)
+        return fixed_v, table, len(rows) + len(tp)
+    split_want = host_split()
+
+    import ctypes as C
+    from zero_chain_b200 import _lib
+    slots, bal, pend, fl = ab.state
+    n, ns = len(ab.txs), len(slots)
+    u8 = lambda b: np.frombuffer(bytes(b), np.uint8).copy()
+    c_in = [np.array([x for x, _ in slots], np.uint32), u8(b"".join(k for _, k in slots)), u8(bal), u8(pend), u8(fl),
+            u8(bytes(t.kind for t in ab.txs)), np.array([t.asset_id if t.kind != zk.ASSET_ISSUE else 0 for t in ab.txs], np.uint32),
+            u8(b"".join(t.verify_points(bytes(64)) if t.kind == zk.ASSET_TRANSFER else t.verify_points() for t in ab.txs)),
+            u8(b"".join(ab.proofs))]
+
+    def c_call():
+        nr = ns + 2 * n
+        out = [np.zeros(m, np.uint8) for m in (n, 4 * n, 64 * n, 128 * n, n, n, 4 * nr, 32 * nr, 64 * nr, 64 * nr, nr)]
+        n_out, rounds = C.c_size_t(0), C.c_uint(0)
+        zk._ck(_lib.lib().zk_import_asset_calls(ctx._h, pvk._h, ns, *[zk._p(x) for x in c_in[:5]], ab.next_asset_id, ab.new_slot_flags, n,
+                                                *[zk._p(x) for x in c_in[5:]], *[zk._p(o) for o in out], C.byref(n_out), C.byref(rounds)))
+        m = n_out.value
+        return (out[0].tobytes(), out[8][:64 * m].tobytes(), out[9][:64 * m].tobytes(), out[10][:m].tobytes(), rounds.value)
+    c_want = (bytes(awant[0]),) + awant[3][1:] + (awant[4],)
+
     def check_assets(k, out):
-        if k == "verify":
+        if k == "calls_c":
+            assert out == c_want, "the C call differs"
+        elif k == "verify":
             assert out == av_want, "verification alone differs"
+        elif k == "split":
+            assert all(np.array_equal(x, y) if isinstance(x, np.ndarray) else x == y for x, y in zip(out[1][1:], split_want[1][1:]))
+            assert out[1][0] == split_want[1][0] and bytes(out[0]) == bytes(split_want[0]) and out[2] == split_want[2]
         else:
             assert out == awant, "%s differs" % k
-    return dict(measure("assets", lambda: zk.import_assets_block(ctx, pvk, *ab.args()), lambda: zk.assets_import(ctx, pvk, *ab.args()),
-                                 verify_alone(ab.rows, ab.proofs), check_assets),
-                n_tx=a.asset_tx, slots=a.slots, rounds=awant[4], failures=sum(v != 1 for v in awant[0]))
+    r = dict(measure("assets", lambda: zk.import_assets_block(ctx, pvk, *ab.args()), lambda: zk.assets_import(ctx, pvk, *ab.args()),
+                     verify_alone(ab.rows, ab.proofs), check_assets,
+                     extra=[("calls", lambda: zk.asset_calls_import(ctx, pvk, *ab.args())), ("calls_c", c_call), ("split", host_split)]),
+             n_tx=a.asset_tx, slots=a.slots, rounds=awant[4], failures=sum(v != 1 for v in awant[0]))
+    # the split arm is host work timed in parts: its medians, not its ratio, are the result
+    r["ms"].pop("split")
+    r.pop("split_over_verify")
+    r["assets_import_host_ms"] = {k: round(float(np.median(v[-a.reps:])), 3) for k, v in split.items()}
+    return r
 
 
 def anonymous_leg(a, ctx, measure):

@@ -89,6 +89,8 @@ SIGNATURES = {
     "zk_import_confidential_block_device": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 10 + [C.POINTER(u32)]),
     "zk_import_assets_block": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 15 + [C.POINTER(u32)]),
     "zk_import_assets_block_device": (i32, [vp, vp, sz, vp, vp, vp, sz] + [vp] * 15 + [C.POINTER(u32)]),
+    "zk_import_asset_calls": (i32, [vp, vp, sz] + [vp] * 5 + [u32, C.c_uint8, sz] + [vp] * 15 + [C.POINTER(sz), C.POINTER(u32)]),
+    "zk_import_asset_calls_device": (i32, [vp, vp, sz] + [vp] * 5 + [u32, C.c_uint8, sz] + [vp] * 15 + [C.POINTER(sz), C.POINTER(u32)]),
     "zk_import_anonymous_block": (i32, [vp, vp, vp, sz, vp, vp, vp, vp, sz] + [vp] * 14),
     "zk_import_anonymous_block_device": (i32, [vp, vp, vp, sz, vp, vp, vp, vp, sz] + [vp] * 14),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),

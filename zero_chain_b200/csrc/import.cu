@@ -6,6 +6,7 @@
 // each round (failures, transfers left undecided), which is all it needs to launch the next round.
 // zk_import_anonymous_block and its _device form (anon_run) take no rounds: a fixed sequence of verifications and state
 // passes (import.cuh section 5), with one read of the counter block to size the two verifications.
+// zk_import_asset_calls and its _device form (asset_calls_run): import.cuh section 6's passes, then assets_run.
 //
 // The round buffers live in the context (ctx->imp); the host forms stage their arrays in ctx->imp_io.
 #include "internal.h"
@@ -74,6 +75,55 @@ static __global__ void __launch_bounds__(BT) k_imp_an_gather(size_t n, const uin
     IMP_FOR(i, n) imp_an_gather(i, kind, pos, verify_points, proofs, rows, round_proofs);
 }
 
+// zk_import_asset_calls
+static __global__ void __launch_bounds__(BT) k_imp_as_start(size_t n_tx, const uint8_t *__restrict__ kind, uint32_t *__restrict__ flag,
+                                                            uint32_t *cnt) {
+    IMP_FOR(k, n_tx) imp_as_start(k, kind, flag, cnt);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_row_insert(size_t n_slots, ImpAsKeys t, uint32_t *table, uint32_t cap) {
+    IMP_FOR(r, n_slots) imp_as_row_insert(r, t, table, cap);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_row_dup(size_t n_slots, ImpAsKeys t, const uint32_t *__restrict__ table, uint32_t cap,
+                                                              uint32_t *cnt) {
+    IMP_FOR(r, n_slots) imp_as_row_dup(r, t, table, cap, cnt);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_compact(size_t n, const uint8_t *__restrict__ kind, const uint32_t *__restrict__ pos,
+                                                              const uint8_t *__restrict__ rows, const uint8_t *__restrict__ proofs,
+                                                              uint8_t *__restrict__ round_rows, uint8_t *__restrict__ round_proofs) {
+    IMP_FOR(i, n) imp_compact(i, IMP_ROW, true, kind, pos, rows, proofs, round_rows, round_proofs);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_issue_flag(size_t n_tx, const uint8_t *__restrict__ kind,
+                                                                 const uint8_t *__restrict__ verdicts, uint32_t *__restrict__ flag) {
+    IMP_FOR(k, n_tx) imp_as_issue_flag(k, kind, verdicts, flag);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_refs(size_t n_tx, uint32_t next_id, const uint8_t *__restrict__ kind,
+                                                           const uint32_t *__restrict__ asset_id, const uint8_t *__restrict__ verdicts,
+                                                           const uint32_t *__restrict__ ipos, uint32_t *__restrict__ asset_ids,
+                                                           uint32_t *__restrict__ ref_id, uint8_t *__restrict__ ref_on, uint32_t *cnt) {
+    IMP_FOR(k, n_tx) imp_as_refs(k, next_id, kind, asset_id, verdicts, ipos, asset_ids, ref_id, ref_on, cnt);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_ref_insert(size_t n_ref, const uint8_t *__restrict__ ref_on, ImpAsKeys t, uint32_t *table,
+                                                                 uint32_t cap) {
+    IMP_FOR(p, n_ref) imp_as_ref_insert(p, ref_on, t, table, cap);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_new(size_t n_ref, const uint8_t *__restrict__ ref_on, ImpAsKeys t,
+                                                          const uint32_t *__restrict__ table, uint32_t cap, uint32_t *__restrict__ flag,
+                                                          uint32_t *cnt) {
+    IMP_FOR(p, n_ref) imp_as_new(p, ref_on, t, table, cap, flag, cnt);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_slot(size_t n_ref, const uint8_t *__restrict__ ref_on, ImpAsKeys t,
+                                                           const uint32_t *__restrict__ table, uint32_t cap, const uint32_t *__restrict__ newpos,
+                                                           uint8_t flags, uint32_t *__restrict__ slot_a, uint32_t *__restrict__ slot_b,
+                                                           uint32_t *__restrict__ new_ids, uint8_t *__restrict__ new_keys,
+                                                           uint8_t *__restrict__ balances, uint8_t *__restrict__ pendings,
+                                                           uint8_t *__restrict__ slot_flags) {
+    IMP_FOR(p, n_ref) imp_as_slot(p, ref_on, t, table, cap, newpos, flags, slot_a, slot_b, new_ids, new_keys, balances, pendings, slot_flags);
+}
+static __global__ void __launch_bounds__(BT) k_imp_as_tx_points(size_t n, const uint8_t *__restrict__ kind, const uint8_t *__restrict__ rows,
+                                                                uint8_t *__restrict__ tx_points) {
+    IMP_FOR(i, n) imp_as_tx_points(i, kind, rows, tx_points);
+}
+
 static unsigned grid(size_t n) { return (unsigned)(n ? (n + BT - 1) / BT : 1); }
 
 struct ImpWork {
@@ -92,8 +142,8 @@ static size_t carve(Carve &c, ImpWork &w, size_t n_tx, size_t n_keys, bool tx_po
 
 // the counter block to the host; zk_check_err_flag synchronises the stream and reports a touched account or slot that
 // failed to read in the state pass
-static int read_counters(zk_ctx *ctx, const uint32_t *d_cnt, uint32_t *cnt) {
-    ZK_CUDA(cudaMemcpyAsync(cnt, d_cnt, IMP_COUNTERS * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+static int read_counters(zk_ctx *ctx, const uint32_t *d_cnt, uint32_t *cnt, size_t n = IMP_COUNTERS) {
+    ZK_CUDA(cudaMemcpyAsync(cnt, d_cnt, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     return zk_check_err_flag(ctx);
 }
 
@@ -367,6 +417,229 @@ extern "C" int zk_import_assets_block(zk_ctx *ctx, const zk_pvk *pvk, size_t n_s
         }
     }
     ZK_CUDA(cudaStreamSynchronize(st));
+    return ZK_OK;
+}
+
+// ---- encrypted-asset calls from the extrinsic fields -------------------------------------------------------------------
+// The passes of import.cuh section 6, then assets_run on the grown table with the issue and destroy verdicts fixed.  The
+// host reads the counter block twice before the rounds: after imp_as_start, since the number of issues and destroys sizes
+// their verification, and after imp_as_slot, since the number of new rows sizes the state pass.
+static_assert(IMP_TRANSFER == zkbal::AS_TRANSFER && IMP_ISSUE == zkbal::AS_ISSUE && IMP_DESTROY == zkbal::AS_DESTROY,
+              "import.cuh's kinds are assets.cuh's");
+
+struct AsWork {
+    uint8_t *round_rows, *round_proofs, *rv, *ref_on, *tx_points, *balances, *pendings, *flags;
+    uint32_t *cnt, *totals, *pos, *ipos, *ref_id, *newpos, *table, *slot_a, *slot_b;
+};
+
+// n_rows = n_slots + 2 n_tx: the table grown by a new row at every reference at most
+static size_t carve(Carve &c, AsWork &w, size_t n_tx, size_t n_rows, size_t cap) {
+    w.cnt = c.take<uint32_t>(IMP_AS_COUNTERS); w.totals = c.take<uint32_t>(PREFIX_TOTALS);
+    w.round_rows = c.take<uint8_t>(IMP_ROW * n_tx); w.round_proofs = c.take<uint8_t>(192 * n_tx); w.rv = c.take<uint8_t>(n_tx);
+    w.pos = c.take<uint32_t>(n_tx); w.ipos = c.take<uint32_t>(n_tx); w.ref_id = c.take<uint32_t>(2 * n_tx); w.ref_on = c.take<uint8_t>(2 * n_tx);
+    w.newpos = c.take<uint32_t>(2 * n_tx); w.table = c.take<uint32_t>(cap); w.slot_a = c.take<uint32_t>(n_tx); w.slot_b = c.take<uint32_t>(n_tx);
+    w.tx_points = c.take<uint8_t>(128 * n_tx);
+    w.balances = c.take<uint8_t>(64 * n_rows); w.pendings = c.take<uint8_t>(64 * n_rows); w.flags = c.take<uint8_t>(n_rows);
+    return c.off;
+}
+
+static int asset_calls_args(const char *fn, zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const void *slot_ids, const void *slot_keys,
+                            const void *balances, const void *pendings, const void *slot_flags, size_t n_tx, const void *kind,
+                            const void *asset_id, const void *rows, const void *proofs, const void *verdicts, const void *asset_ids,
+                            const void *balance_after, const void *event_ct, const void *event_flags, const void *tx_status,
+                            const void *new_slot_ids, const void *new_slot_keys, const void *new_balances, const void *new_pendings,
+                            const void *new_flags, const void *n_slots_out) {
+    if (!ctx || !pvk || !n_slots_out || (n_slots && (!slot_ids || !slot_keys || !balances || !pendings || !slot_flags)) ||
+        (n_tx && (!kind || !asset_id || !rows || !proofs || !verdicts || !asset_ids || !balance_after || !event_ct || !event_flags ||
+                  !tx_status)) ||
+        ((n_slots || n_tx) && (!new_slot_ids || !new_slot_keys || !new_balances || !new_pendings || !new_flags))) {
+        zk_set_error("%s: NULL argument", fn);
+        return ZK_ERR_INVALID;
+    }
+    if (n_slots > zkbal::BAL_MAX || n_tx > zkbal::AS_MAX_TX) {
+        zk_set_error("%s: n_slots = %zu, n_tx = %zu: at most %u slots and %u transactions", fn, n_slots, n_tx, zkbal::BAL_MAX,
+                     zkbal::AS_MAX_TX);
+        return ZK_ERR_INVALID;
+    }
+    return ZK_OK;
+}
+
+// All arrays are device pointers; the table outputs have room for n_slots + 2 n_tx rows.
+static int asset_calls_run(zk_ctx *ctx, const char *fn, const zk_pvk *pvk, size_t n_slots, const uint32_t *slot_ids, const uint8_t *slot_keys,
+                           const uint8_t *balances, const uint8_t *pendings, const uint8_t *slot_flags, uint32_t next_asset_id,
+                           uint8_t new_slot_flags, size_t n_tx, const uint8_t *kind, const uint32_t *asset_id, const uint8_t *rows,
+                           const uint8_t *proofs, uint8_t *verdicts, uint32_t *asset_ids, uint8_t *balance_after, uint8_t *event_ct,
+                           uint8_t *event_flags, uint8_t *tx_status, uint32_t *new_slot_ids, uint8_t *new_slot_keys, uint8_t *new_balances,
+                           uint8_t *new_pendings, uint8_t *new_flags, size_t *n_slots_out, unsigned *rounds) {
+    cudaStream_t st = ctx->stream;
+    const size_t n_ref = 2 * n_tx, n_rows = n_slots + n_ref, cap = ZK_IAS_CAPACITY(n_rows);
+    AsWork w;
+    Carve sizing;
+    ZK_TRY(ctx->imp_as.reserve(carve(sizing, w, n_tx, n_rows, cap)));
+    Carve c;
+    c.base = ctx->imp_as.as<uint8_t>();
+    carve(c, w, n_tx, n_rows, cap);
+    const ImpAsKeys keys{slot_ids, slot_keys, w.ref_id, rows, (uint32_t)n_slots};
+    uint32_t cnt[IMP_AS_COUNTERS];
+
+    // 1. kinds, and the table's rows into the hash table
+    ZK_CUDA(cudaMemsetAsync(w.cnt, 0, IMP_AS_BAD * sizeof(uint32_t), st));
+    ZK_CUDA(cudaMemsetAsync(w.cnt + IMP_AS_BAD, 0xFF, (IMP_AS_COUNTERS - IMP_AS_BAD) * sizeof(uint32_t), st));
+    ZK_CUDA(cudaMemsetAsync(w.table, 0xFF, cap * sizeof(uint32_t), st));
+    if (n_tx) k_imp_as_start<<<grid(n_tx), BT, 0, st>>>(n_tx, kind, w.pos, w.cnt);
+    k_imp_as_row_insert<<<grid(n_slots), BT, 0, st>>>(n_slots, keys, w.table, (uint32_t)cap);
+    k_imp_as_row_dup<<<grid(n_slots), BT, 0, st>>>(n_slots, keys, w.table, (uint32_t)cap, w.cnt);
+    ZK_CUDA(cudaGetLastError());
+    ZK_TRY(read_counters(ctx, w.cnt, cnt, IMP_AS_COUNTERS));
+    if (cnt[IMP_AS_BAD] != IMP_NONE) {
+        zk_set_error("%s: transaction %u: an unknown kind", fn, cnt[IMP_AS_BAD]);
+        return ZK_ERR_INVALID;
+    }
+    if (cnt[IMP_AS_DUP] != IMP_NONE) {
+        zk_set_error("%s: slot row %u repeats an earlier row's (asset id, key)", fn, cnt[IMP_AS_DUP]);
+        return ZK_ERR_INVALID;
+    }
+
+    if (n_tx) {
+        // 2. the issues and destroys, verified; their verdicts fixed (transfers 0 until the rounds start them)
+        const size_t m = cnt[IMP_AS_FIXED];
+        ZK_CUDA(cudaMemsetAsync(verdicts, 0, n_tx, st));
+        if (m) {
+            ZK_TRY(zk_bal_prefix_sum(ctx, w.pos, n_tx, w.totals));
+            k_imp_as_compact<<<grid(IMP_WORDS * n_tx), BT, 0, st>>>(IMP_WORDS * n_tx, kind, w.pos, rows, proofs, w.round_rows, w.round_proofs);
+            ZK_CUDA(cudaGetLastError());
+            ZK_TRY(zk_groth16_verify_points_batch_device(ctx, pvk, m, w.round_proofs, w.round_rows, IMP_POINTS, w.rv));
+            k_imp_an_scatter<<<grid(n_tx), BT, 0, st>>>(n_tx, true, kind, w.pos, w.rv, verdicts);
+        }
+        // 3. asset ids and references
+        k_imp_as_issue_flag<<<grid(n_tx), BT, 0, st>>>(n_tx, kind, verdicts, w.ipos);
+        ZK_CUDA(cudaGetLastError());
+        ZK_TRY(zk_bal_prefix_sum(ctx, w.ipos, n_tx, w.totals));
+        k_imp_as_refs<<<grid(n_tx), BT, 0, st>>>(n_tx, next_asset_id, kind, asset_id, verdicts, w.ipos, asset_ids, w.ref_id, w.ref_on, w.cnt);
+        // 4. the references into the hash table; new rows numbered in the order of their first reference
+        k_imp_as_ref_insert<<<grid(n_ref), BT, 0, st>>>(n_ref, w.ref_on, keys, w.table, (uint32_t)cap);
+        k_imp_as_new<<<grid(n_ref), BT, 0, st>>>(n_ref, w.ref_on, keys, w.table, (uint32_t)cap, w.newpos, w.cnt);
+        ZK_CUDA(cudaGetLastError());
+        ZK_TRY(zk_bal_prefix_sum(ctx, w.newpos, n_ref, w.totals));
+    }
+    // the table's rows, then the new ones behind them
+    if (n_slots) {
+        ZK_CUDA(cudaMemcpyAsync(w.balances, balances, 64 * n_slots, cudaMemcpyDeviceToDevice, st));
+        ZK_CUDA(cudaMemcpyAsync(w.pendings, pendings, 64 * n_slots, cudaMemcpyDeviceToDevice, st));
+        ZK_CUDA(cudaMemcpyAsync(w.flags, slot_flags, n_slots, cudaMemcpyDeviceToDevice, st));
+        ZK_CUDA(cudaMemcpyAsync(new_slot_ids, slot_ids, 4 * n_slots, cudaMemcpyDeviceToDevice, st));
+        ZK_CUDA(cudaMemcpyAsync(new_slot_keys, slot_keys, 32 * n_slots, cudaMemcpyDeviceToDevice, st));
+    }
+    if (n_tx) {
+        const uint8_t flags = (uint8_t)(new_slot_flags & ~(zkbal::ACCT_BALANCE | zkbal::ACCT_PENDING));
+        k_imp_as_slot<<<grid(n_ref), BT, 0, st>>>(n_ref, w.ref_on, keys, w.table, (uint32_t)cap, w.newpos, flags, w.slot_a, w.slot_b,
+                                                  new_slot_ids, new_slot_keys, w.balances, w.pendings, w.flags);
+        k_imp_as_tx_points<<<grid(32 * n_tx), BT, 0, st>>>(32 * n_tx, kind, rows, w.tx_points);
+        ZK_CUDA(cudaGetLastError());
+        ZK_TRY(read_counters(ctx, w.cnt, cnt, IMP_AS_COUNTERS));
+        if (cnt[IMP_AS_OVF] != IMP_NONE) {
+            zk_set_error("%s: transaction %u: the issue's asset id would pass 2^32 - 1", fn, cnt[IMP_AS_OVF]);
+            return ZK_ERR_INVALID;
+        }
+    }
+    const size_t ns = n_slots + cnt[IMP_AS_NEW];
+    if (ns > zkbal::BAL_MAX) {
+        zk_set_error("%s: %zu slots after the block's new ones: at most %u", fn, ns, zkbal::BAL_MAX);
+        return ZK_ERR_INVALID;
+    }
+    *n_slots_out = ns;
+    // 5. the rounds, the issue and destroy verdicts fixed in verdicts itself
+    return assets_run(ctx, fn, pvk, ns, w.balances, w.pendings, w.flags, n_tx, kind, w.slot_a, w.slot_b, w.tx_points, rows, proofs, verdicts,
+                      verdicts, balance_after, event_ct, event_flags, tx_status, new_balances, new_pendings, new_flags, rounds);
+}
+
+extern "C" int zk_import_asset_calls_device(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const uint32_t *d_slot_ids,
+                                            const uint8_t *d_slot_keys, const uint8_t *d_balances, const uint8_t *d_pendings,
+                                            const uint8_t *d_slot_flags, uint32_t next_asset_id, uint8_t new_slot_flags, size_t n_tx,
+                                            const uint8_t *d_kind, const uint32_t *d_asset_id, const uint8_t *d_rows, const uint8_t *d_proofs,
+                                            uint8_t *d_verdicts, uint32_t *d_asset_ids, uint8_t *d_balance_after, uint8_t *d_event_ct,
+                                            uint8_t *d_event_flags, uint8_t *d_tx_status, uint32_t *d_new_slot_ids, uint8_t *d_new_slot_keys,
+                                            uint8_t *d_new_balances, uint8_t *d_new_pendings, uint8_t *d_new_flags, size_t *n_slots_out,
+                                            unsigned *rounds) {
+    const char *fn = "zk_import_asset_calls_device";
+    ZK_TRY(asset_calls_args(fn, ctx, pvk, n_slots, d_slot_ids, d_slot_keys, d_balances, d_pendings, d_slot_flags, n_tx, d_kind, d_asset_id,
+                            d_rows, d_proofs, d_verdicts, d_asset_ids, d_balance_after, d_event_ct, d_event_flags, d_tx_status, d_new_slot_ids,
+                            d_new_slot_keys, d_new_balances, d_new_pendings, d_new_flags, n_slots_out));
+    ZK_TRY(check_key(ctx, pvk));
+    if (rounds) *rounds = 0;
+    *n_slots_out = 0;
+    if (!n_slots && !n_tx) return ZK_OK;
+    ZK_TRY(zk_use_device(ctx));
+    return asset_calls_run(ctx, fn, pvk, n_slots, d_slot_ids, d_slot_keys, d_balances, d_pendings, d_slot_flags, next_asset_id, new_slot_flags,
+                           n_tx, d_kind, d_asset_id, d_rows, d_proofs, d_verdicts, d_asset_ids, d_balance_after, d_event_ct, d_event_flags,
+                           d_tx_status, d_new_slot_ids, d_new_slot_keys, d_new_balances, d_new_pendings, d_new_flags, n_slots_out, rounds);
+}
+
+extern "C" int zk_import_asset_calls(zk_ctx *ctx, const zk_pvk *pvk, size_t n_slots, const uint32_t *slot_ids, const uint8_t *slot_keys,
+                                     const uint8_t *balances, const uint8_t *pendings, const uint8_t *slot_flags, uint32_t next_asset_id,
+                                     uint8_t new_slot_flags, size_t n_tx, const uint8_t *kind, const uint32_t *asset_id, const uint8_t *rows,
+                                     const uint8_t *proofs, uint8_t *verdicts, uint32_t *asset_ids, uint8_t *balance_after, uint8_t *event_ct,
+                                     uint8_t *event_flags, uint8_t *tx_status, uint32_t *new_slot_ids, uint8_t *new_slot_keys,
+                                     uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags, size_t *n_slots_out,
+                                     unsigned *rounds) {
+    const char *fn = "zk_import_asset_calls";
+    ZK_TRY(asset_calls_args(fn, ctx, pvk, n_slots, slot_ids, slot_keys, balances, pendings, slot_flags, n_tx, kind, asset_id, rows, proofs,
+                            verdicts, asset_ids, balance_after, event_ct, event_flags, tx_status, new_slot_ids, new_slot_keys, new_balances,
+                            new_pendings, new_flags, n_slots_out));
+    ZK_TRY(check_key(ctx, pvk));
+    if (rounds) *rounds = 0;
+    *n_slots_out = 0;
+    if (!n_slots && !n_tx) return ZK_OK;
+    ZK_TRY(zk_use_device(ctx));
+    cudaStream_t st = ctx->stream;
+    const size_t ns = n_slots, nr = n_slots + 2 * n_tx;
+    Carve c;
+    for (int pass = 0; pass < 2; pass++) {     // inputs, then outputs
+        if (pass) c = Carve{ctx->imp_io.as<uint8_t>(), 0};
+        uint32_t *si = c.take<uint32_t>(ns);
+        uint8_t *sk = c.take<uint8_t>(32 * ns), *b = c.take<uint8_t>(64 * ns), *p = c.take<uint8_t>(64 * ns), *f = c.take<uint8_t>(ns),
+                *kd = c.take<uint8_t>(n_tx);
+        uint32_t *ai = c.take<uint32_t>(n_tx);
+        uint8_t *rw = c.take<uint8_t>(IMP_ROW * n_tx), *pf = c.take<uint8_t>(192 * n_tx), *v = c.take<uint8_t>(n_tx);
+        uint32_t *ids = c.take<uint32_t>(n_tx);
+        uint8_t *ba = c.take<uint8_t>(64 * n_tx), *ev = c.take<uint8_t>(128 * n_tx), *ef = c.take<uint8_t>(n_tx), *ts = c.take<uint8_t>(n_tx);
+        uint32_t *nsi = c.take<uint32_t>(nr);
+        uint8_t *nsk = c.take<uint8_t>(32 * nr), *nb = c.take<uint8_t>(64 * nr), *npd = c.take<uint8_t>(64 * nr), *nf = c.take<uint8_t>(nr);
+        if (!pass) { ZK_TRY(ctx->imp_io.reserve(c.off)); continue; }
+        if (ns) {
+            ZK_CUDA(cudaMemcpyAsync(si, slot_ids, 4 * ns, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(sk, slot_keys, 32 * ns, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(b, balances, 64 * ns, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(p, pendings, 64 * ns, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(f, slot_flags, ns, cudaMemcpyHostToDevice, st));
+        }
+        if (n_tx) {
+            ZK_CUDA(cudaMemcpyAsync(kd, kind, n_tx, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(ai, asset_id, 4 * n_tx, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(rw, rows, IMP_ROW * n_tx, cudaMemcpyHostToDevice, st));
+            ZK_CUDA(cudaMemcpyAsync(pf, proofs, 192 * n_tx, cudaMemcpyHostToDevice, st));
+        }
+        size_t n_out = 0;
+        ZK_TRY(asset_calls_run(ctx, fn, pvk, ns, si, sk, b, p, f, next_asset_id, new_slot_flags, n_tx, kd, ai, rw, pf, v, ids, ba, ev, ef, ts,
+                               nsi, nsk, nb, npd, nf, &n_out, rounds));
+        if (n_tx) {
+            ZK_CUDA(cudaMemcpyAsync(verdicts, v, n_tx, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(asset_ids, ids, 4 * n_tx, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(balance_after, ba, 64 * n_tx, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(event_ct, ev, 128 * n_tx, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(event_flags, ef, n_tx, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(tx_status, ts, n_tx, cudaMemcpyDeviceToHost, st));
+        }
+        if (n_out) {
+            ZK_CUDA(cudaMemcpyAsync(new_slot_ids, nsi, 4 * n_out, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(new_slot_keys, nsk, 32 * n_out, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(new_balances, nb, 64 * n_out, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(new_pendings, npd, 64 * n_out, cudaMemcpyDeviceToHost, st));
+            ZK_CUDA(cudaMemcpyAsync(new_flags, nf, n_out, cudaMemcpyDeviceToHost, st));
+        }
+        ZK_CUDA(cudaStreamSynchronize(st));
+        *n_slots_out = n_out;
+    }
     return ZK_OK;
 }
 

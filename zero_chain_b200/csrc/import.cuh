@@ -22,9 +22,12 @@
 //      (zk_anonymous_calls_block) with verdicts as the mask,
 //   4. imp_an_gather: each transfer's 52 points from that pass and its proof, verified with the anonymous key,
 //   5. imp_an_scatter: the transfer verdicts, then the state pass again.
+// zk_import_asset_calls (section 6) puts the asset numbering and the slot resolution in front of zk_import_assets_block's
+// rounds.
 //
 // Plain integer code, one function per item and thread of each pass; the same source compiles with ZK_HOST_EMUL for the
-// CPU tests (tests/host_emul/emul_import.cpp, emul_import_anon.cpp), which run the passes as loops over the items.
+// CPU tests (tests/host_emul/emul_import.cpp, emul_import_anon.cpp, emul_import_assets.cpp), which run the passes as loops
+// over the items.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -218,35 +221,219 @@ ZK_IMP_DEV void imp_an_issue_row(size_t i, const uint8_t *kind, const uint32_t *
     for (int b = 0; b < 4; b++) dst[b] = src[b];
 }
 
-// issues: verdicts[k] = rv[pos[k]] at an issue and 0 at a transfer (not applied in the first state pass); otherwise
-// verdicts[k] = rv[k - pos[k]] at a transfer, issues unchanged.
+// pos is the exclusive prefix sum of the flags "not a transfer" (an anonymous issue; an asset issue or destroy), so
+// pos[k] is such a transaction's compact row and k - pos[k] a transfer's.
+// issues: verdicts[k] = rv[pos[k]] at a non-transfer and 0 at a transfer (not applied in the first state pass); otherwise
+// verdicts[k] = rv[k - pos[k]] at a transfer, the others unchanged.
 ZK_IMP_DEV void imp_an_scatter(size_t k, bool issues, const uint8_t *kind, const uint32_t *pos, const uint8_t *rv, uint8_t *verdicts) {
-    const bool issue = kind[k] == IMP_AN_ISSUE;
+    const bool issue = kind[k] != IMP_AN_TRANSFER;
     if (issues)
         verdicts[k] = issue ? rv[pos[k]] : 0;
     else if (!issue)
         verdicts[k] = rv[k - pos[k]];
 }
 
+// Item i: word o / 4 of transaction k's row_bytes-byte row (src_rows) and 192-byte proof, when k is a non-transfer (issues)
+// or a transfer (!issues): into compact row pos[k] or k - pos[k] of rows / round_proofs.
+ZK_IMP_DEV void imp_compact(size_t i, uint32_t row_bytes, bool issues, const uint8_t *kind, const uint32_t *pos, const uint8_t *src_rows,
+                            const uint8_t *proofs, uint8_t *rows, uint8_t *round_proofs) {
+    const uint32_t words = (row_bytes + 192) / 4;
+    const size_t k = i / words;
+    const uint32_t o = 4 * (uint32_t)(i % words);
+    if ((kind[k] != IMP_AN_TRANSFER) != issues) return;
+    const size_t j = issues ? pos[k] : k - pos[k];
+    const uint8_t *src;
+    uint8_t *dst;
+    if (o < row_bytes) {
+        src = src_rows + (size_t)row_bytes * k + o;
+        dst = rows + (size_t)row_bytes * j + o;
+    } else {
+        src = proofs + 192 * k + (o - row_bytes);
+        dst = round_proofs + 192 * j + (o - row_bytes);
+    }
+#pragma unroll
+    for (int b = 0; b < 4; b++) dst[b] = src[b];
+}
+
 // Item i: word w = i % IMP_AN_WORDS of transaction k = i / IMP_AN_WORDS, when k is a transfer: words [0, 416) are its 52
 // points from the state pass's verify_points, words [416, 464) its proof, into row k - pos[k].
 ZK_IMP_DEV void imp_an_gather(size_t i, const uint8_t *kind, const uint32_t *pos, const uint8_t *verify_points, const uint8_t *proofs,
                               uint8_t *rows, uint8_t *round_proofs) {
-    const size_t k = i / IMP_AN_WORDS;
-    const uint32_t o = 4 * (uint32_t)(i % IMP_AN_WORDS);
-    if (kind[k] != IMP_AN_TRANSFER) return;
-    const size_t j = k - pos[k];
-    const uint8_t *src;
-    uint8_t *dst;
-    if (o < IMP_AN_ROW) {
-        src = verify_points + IMP_AN_ROW * k + o;
-        dst = rows + IMP_AN_ROW * j + o;
-    } else {
-        src = proofs + 192 * k + (o - IMP_AN_ROW);
-        dst = round_proofs + 192 * j + (o - IMP_AN_ROW);
+    imp_compact(i, IMP_AN_ROW, false, kind, pos, verify_points, proofs, rows, round_proofs);
+}
+
+// ---- 6. zk_import_asset_calls ------------------------------------------------------------------------------------------
+// The passes in front of zk_import_assets_block's rounds, from the slot table as the module stores it and the extrinsic
+// fields (import.cu's asset_calls_run):
+//   1. imp_as_start: check each kind, flag the issues and destroys; imp_as_row_insert / imp_as_row_dup: the table's rows
+//      into the hash table, and the lowest row whose key repeats an earlier row's.  The host reads the counter block.
+//   2. zk_bal_prefix_sum + imp_compact: the issue and destroy rows and proofs, verified; imp_an_scatter: their verdicts.
+//   3. imp_as_issue_flag + zk_bal_prefix_sum: each passing issue's number among them; imp_as_refs: its asset id, and the
+//      (asset id, key) every transaction references at positions 2k (slot_a) and 2k + 1 (slot_b).
+//   4. imp_as_ref_insert: the references into the hash table; imp_as_new + zk_bal_prefix_sum: each new key's row, in the
+//      order of its first reference; imp_as_slot: slot_a / slot_b, and each new row's (id, key), zero ciphertexts and flags.
+//      imp_as_tx_points: the state pass's tx_points.  The host reads the counter block again (new rows, id overflow).
+// The hash table: open addressing with linear probing over `cap` uint32 entries, IMP_NONE when empty.  An entry holds a
+// handle: r < n_slots is table row r, n_slots + p is reference p.  Inserting a handle whose key is present lowers the
+// entry to the least handle of that key (imp_min), so once every insert is done the entry is the key's table row if it
+// has one, and its first reference otherwise, whatever order the threads ran in.  Keys are compared in full.
+constexpr uint8_t IMP_ISSUE = 1;
+constexpr uint32_t IMP_ASSET_ID_MAX = 0xFFFFFFFFu;
+// the counter block of zk_import_asset_calls: the issues and destroys, the new rows, and the lowest transaction with an
+// unknown kind, table row repeating an earlier one, and passing issue whose id would pass IMP_ASSET_ID_MAX
+enum ImpAsCounter { IMP_AS_FIXED = 0, IMP_AS_NEW = 1, IMP_AS_BAD = 2, IMP_AS_DUP = 3, IMP_AS_OVF = 4, IMP_AS_COUNTERS = 5 };
+
+// the keys behind the handles: a table row's (slot_ids[r], slot_keys[r]); reference p's (ref_id[p], slot p & 1 of row p / 2)
+struct ImpAsKeys {
+    const uint32_t *slot_ids;
+    const uint8_t *slot_keys;
+    const uint32_t *ref_id;
+    const uint8_t *rows;
+    uint32_t n_slots;
+};
+ZK_IMP_DEV uint32_t imp_as_id(const ImpAsKeys &t, uint32_t h) { return h < t.n_slots ? t.slot_ids[h] : t.ref_id[h - t.n_slots]; }
+ZK_IMP_DEV const uint8_t *imp_as_key(const ImpAsKeys &t, uint32_t h) {
+    if (h < t.n_slots) return t.slot_keys + 32 * (size_t)h;
+    const uint32_t p = h - t.n_slots;
+    return t.rows + IMP_ROW * (size_t)(p >> 1) + 32 * (p & 1);
+}
+ZK_IMP_DEV bool imp_as_equal(const ImpAsKeys &t, uint32_t a, uint32_t b) {
+    if (imp_as_id(t, a) != imp_as_id(t, b)) return false;
+    const uint8_t *x = imp_as_key(t, a), *y = imp_as_key(t, b);
+    uint32_t diff = 0;
+    for (int i = 0; i < 32; i++) diff |= x[i] ^ y[i];
+    return !diff;
+}
+// FNV-1a over the id's 4 little-endian bytes and the key's 32, then murmur3's finaliser
+ZK_IMP_DEV uint32_t imp_as_hash(uint32_t id, const uint8_t *key) {
+    uint32_t h = 2166136261u;
+    for (int i = 0; i < 4; i++) h = (h ^ ((id >> (8 * i)) & 0xFF)) * 16777619u;
+    for (int i = 0; i < 32; i++) h = (h ^ key[i]) * 16777619u;
+    h ^= h >> 16; h *= 0x85ebca6bu; h ^= h >> 13; h *= 0xc2b2ae35u; h ^= h >> 16;
+    return h;
+}
+// entries for n keys: a power of two, at most half full
+inline size_t imp_as_capacity(size_t n) {
+    size_t c = 64;
+    while (c < 2 * n) c <<= 1;
+    return c;
+}
+// The emulation build may override both, e.g. a constant hash and n + 1 entries put every key into one probe chain.
+#ifndef ZK_IAS_HASH
+#define ZK_IAS_HASH(id, key) imp_as_hash(id, key)
+#endif
+#ifndef ZK_IAS_CAPACITY
+#define ZK_IAS_CAPACITY(n) imp_as_capacity(n)
+#endif
+
+ZK_IMP_DEV uint32_t imp_cas(uint32_t *p, uint32_t cmp, uint32_t v) {
+#ifdef ZK_HOST_EMUL
+    const uint32_t old = *p;
+    if (old == cmp) *p = v;
+    return old;
+#else
+    return atomicCAS(p, cmp, v);
+#endif
+}
+ZK_IMP_DEV uint32_t imp_as_first(const ImpAsKeys &t, uint32_t h, uint32_t cap) {
+    return (uint32_t)(ZK_IAS_HASH(imp_as_id(t, h), imp_as_key(t, h)) % cap);
+}
+// handle h into the table (cap > the number of distinct keys, so an empty entry is always ahead)
+ZK_IMP_DEV void imp_as_insert(const ImpAsKeys &t, uint32_t h, uint32_t *table, uint32_t cap) {
+    for (uint32_t e = imp_as_first(t, h, cap);; e = e + 1 == cap ? 0 : e + 1) {
+        const uint32_t cur = imp_cas(table + e, IMP_NONE, h);
+        if (cur == IMP_NONE) return;
+        if (imp_as_equal(t, cur, h)) {
+            imp_min(table + e, h);
+            return;
+        }
+    }
+}
+// after every insert: the entry of h's key (IMP_NONE for a key never inserted)
+ZK_IMP_DEV uint32_t imp_as_find(const ImpAsKeys &t, uint32_t h, const uint32_t *table, uint32_t cap) {
+    for (uint32_t e = imp_as_first(t, h, cap);; e = e + 1 == cap ? 0 : e + 1) {
+        const uint32_t cur = table[e];
+        if (cur == IMP_NONE || imp_as_equal(t, cur, h)) return cur;
+    }
+}
+
+// an unknown kind puts k in cnt[IMP_AS_BAD]; flag[k] = 1 for an issue or destroy, counted in cnt[IMP_AS_FIXED]
+ZK_IMP_DEV void imp_as_start(size_t k, const uint8_t *kind, uint32_t *flag, uint32_t *cnt) {
+    const uint8_t kd = kind[k];
+    if (kd > IMP_DESTROY) imp_min(cnt + IMP_AS_BAD, (uint32_t)k);
+    flag[k] = kd == IMP_ISSUE || kd == IMP_DESTROY;
+    if (flag[k]) imp_inc(cnt + IMP_AS_FIXED);
+}
+ZK_IMP_DEV void imp_as_row_insert(size_t r, const ImpAsKeys &t, uint32_t *table, uint32_t cap) { imp_as_insert(t, (uint32_t)r, table, cap); }
+// after every row insert: a row whose entry holds an earlier row repeats that row's key
+ZK_IMP_DEV void imp_as_row_dup(size_t r, const ImpAsKeys &t, const uint32_t *table, uint32_t cap, uint32_t *cnt) {
+    if (imp_as_find(t, (uint32_t)r, table, cap) != r) imp_min(cnt + IMP_AS_DUP, (uint32_t)r);
+}
+
+// flag[k] = 1 for a passing issue; zk_bal_prefix_sum turns the flags into the passing issues before k
+ZK_IMP_DEV void imp_as_issue_flag(size_t k, const uint8_t *kind, const uint8_t *verdicts, uint32_t *flag) {
+    flag[k] = kind[k] == IMP_ISSUE && verdicts[k] == 1;
+}
+// The references of transaction k and a passing issue's id, next_id + ipos[k]; one past IMP_ASSET_ID_MAX puts k in
+// cnt[IMP_AS_OVF].  asset_ids[k] is that id at a passing issue and 0 elsewhere.  Reference 2k: a transfer's (asset_id,
+// sender), a passing issue's (id, issuer), a passing destroy's (asset_id, owner); 2k + 1: a transfer's (asset_id,
+// recipient).  ref_on[p] = 0 where there is none.
+ZK_IMP_DEV void imp_as_refs(size_t k, uint32_t next_id, const uint8_t *kind, const uint32_t *asset_id, const uint8_t *verdicts,
+                            const uint32_t *ipos, uint32_t *asset_ids, uint32_t *ref_id, uint8_t *ref_on, uint32_t *cnt) {
+    const uint8_t kd = kind[k];
+    const bool pass = verdicts[k] == 1;
+    uint32_t id = asset_id[k], issued = 0;
+    if (kd == IMP_ISSUE && pass) {
+        const uint64_t v = (uint64_t)next_id + ipos[k];
+        if (v > IMP_ASSET_ID_MAX) imp_min(cnt + IMP_AS_OVF, (uint32_t)k);
+        id = issued = (uint32_t)v;
+    }
+    asset_ids[k] = issued;
+    ref_id[2 * k] = ref_id[2 * k + 1] = id;
+    ref_on[2 * k] = kd == IMP_TRANSFER || pass;
+    ref_on[2 * k + 1] = kd == IMP_TRANSFER;
+}
+ZK_IMP_DEV void imp_as_ref_insert(size_t p, const uint8_t *ref_on, const ImpAsKeys &t, uint32_t *table, uint32_t cap) {
+    if (ref_on[p]) imp_as_insert(t, t.n_slots + (uint32_t)p, table, cap);
+}
+// after every reference insert: flag[p] = 1 where reference p is its key's first and the key is in no table row, counted
+// in cnt[IMP_AS_NEW]; zk_bal_prefix_sum turns the flags into each new key's row past n_slots
+ZK_IMP_DEV void imp_as_new(size_t p, const uint8_t *ref_on, const ImpAsKeys &t, const uint32_t *table, uint32_t cap, uint32_t *flag,
+                           uint32_t *cnt) {
+    const uint32_t h = t.n_slots + (uint32_t)p;
+    flag[p] = ref_on[p] && imp_as_find(t, h, table, cap) == h;
+    if (flag[p]) imp_inc(cnt + IMP_AS_NEW);
+}
+// reference p's slot into slot_a[p / 2] (p even) or slot_b[p / 2] (IMP_NONE: no reference).  A new key's first reference
+// also writes its row: (id, key) into new_ids / new_keys, zero ciphertexts into balances / pendings, and flags.
+ZK_IMP_DEV void imp_as_slot(size_t p, const uint8_t *ref_on, const ImpAsKeys &t, const uint32_t *table, uint32_t cap, const uint32_t *newpos,
+                            uint8_t flags, uint32_t *slot_a, uint32_t *slot_b, uint32_t *new_ids, uint8_t *new_keys, uint8_t *balances,
+                            uint8_t *pendings, uint8_t *slot_flags) {
+    uint32_t slot = IMP_NONE;
+    if (ref_on[p]) {
+        const uint32_t h = t.n_slots + (uint32_t)p, e = imp_as_find(t, h, table, cap);
+        slot = e < t.n_slots ? e : t.n_slots + newpos[e - t.n_slots];
+        if (e == h) {
+            const uint8_t *key = imp_as_key(t, h);
+            new_ids[slot] = t.ref_id[p];
+            for (int i = 0; i < 32; i++) new_keys[32 * (size_t)slot + i] = key[i];
+            for (int i = 0; i < 64; i++) balances[64 * (size_t)slot + i] = pendings[64 * (size_t)slot + i] = 0;
+            slot_flags[slot] = flags;
+        }
+    }
+    (p & 1 ? slot_b : slot_a)[p >> 1] = slot;
+}
+// zk_assets_block's tx_points: a transfer's as imp_tx_points; an issue's total | 0 | 0 | randomness (slots 2 and 4); a
+// destroy's zero
+ZK_IMP_DEV void imp_as_tx_points(size_t i, const uint8_t *kind, const uint8_t *rows, uint8_t *tx_points) {
+    const uint8_t kd = kind[i >> 5];
+    const uint32_t at = (uint32_t)(i & 31) >> 3;
+    if (kd == IMP_TRANSFER || (kd == IMP_ISSUE && (at == 0 || at == 3))) {
+        imp_tx_points(i, rows, tx_points);
+        return;
     }
 #pragma unroll
-    for (int b = 0; b < 4; b++) dst[b] = src[b];
+    for (int b = 0; b < 4; b++) tx_points[4 * i + b] = 0;
 }
 
 }  // namespace zkimp

@@ -89,6 +89,7 @@ struct zk_ctx {
                                    // (anon_balances.cu) and zk_assets_block (assets.cu): workspace, and the host forms' staging
     DevBuf imp, imp_io;            // zk_import_confidential_block / zk_import_assets_block (import.cu): round buffers, and
                                    // the host forms' staging
+    DevBuf imp_as;                 // zk_import_asset_calls (import.cu): the hash table, references and grown slot table
     DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;

@@ -1245,6 +1245,69 @@ def assets_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: int, 
     return rounds.value
 
 
+def asset_calls_import(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
+    """import_assets_block in one call (zk_import_asset_calls): the issue and destroy verification, the asset numbering, the
+    slot resolution and the transfer rounds all run on the device between one upload and one download, with the proofs
+    checked on ctx.  Same arguments, result and errors, plus a ValueError for a slot table that holds one (asset id, key)
+    twice; a key of another shape raises as confidential_import does.  Asset ids (and next_asset_id) are AssetId = u32."""
+    slots, balances, pendings, flags = state
+    slots = [(int(a), _pt32(k)) for a, k in slots]
+    n, ns = len(txs), len(slots)
+    proofs = _cat(proofs, 192)
+    assert len(proofs) == 192 * n and len(flags) == ns
+    ids = [a for a, _ in slots] + [t.asset_id for t in txs if t.kind != ASSET_ISSUE] + [int(next_asset_id)]
+    if any(not 0 <= a <= ASSET_ID_MAX for a in ids):
+        raise ValueError("asset_calls_import: asset id out of range")
+    rows = b"".join(t.verify_points(bytes(64)) if t.kind == ASSET_TRANSFER else t.verify_points() for t in txs)
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    u32 = lambda a: np.array(a or [0], np.uint32)
+    z = lambda m: np.zeros(max(m, 1), np.uint8)
+    nr = ns + 2 * n
+    v, aid, ba, ev, ef, st = z(n), u32([0] * n), z(64 * n), z(128 * n), z(n), z(n)
+    nsi, nsk, nb, npd, nf = u32([0] * nr), z(32 * nr), z(64 * nr), z(64 * nr), z(nr)
+    n_out, rounds = C.c_size_t(0), C.c_uint(0)
+    if pvk.ctx is not ctx:
+        pvk.ctx.sync()
+    try:
+        _ck(_lib.lib().zk_import_asset_calls(ctx._h, pvk._h, ns, _p(u32([a for a, _ in slots])), _p(buf(b"".join(k for _, k in slots))),
+                                             _p(buf(_cat(balances, 64))), _p(buf(_cat(pendings, 64))), _p(buf(bytes(flags))),
+                                             int(next_asset_id), new_slot_flags & 0xFF, n, _p(buf(bytes(t.kind for t in txs))),
+                                             _p(u32([t.asset_id if t.kind != ASSET_ISSUE else 0 for t in txs])), _p(buf(rows)),
+                                             _p(buf(proofs)), _p(v), _p(aid), _p(ba), _p(ev), _p(ef), _p(st), _p(nsi), _p(nsk), _p(nb),
+                                             _p(npd), _p(nf), C.byref(n_out), C.byref(rounds)))
+    except ZkError as e:
+        if e.code == -2 and ("2^32 - 1" in str(e) or "repeats" in str(e)):
+            raise ValueError("asset_calls_import: %s" % e) from None
+        raise
+    m = n_out.value
+    kinds = bytes(t.kind for t in txs)
+    verdicts = [int(x) for x in v[:n]]
+    asset_ids = [int(aid[k]) if kinds[k] == ASSET_ISSUE and verdicts[k] == 1 else None for k in range(n)]
+    events = _asset_events(kinds, ba[:64 * n].tobytes(), ev[:128 * n].tobytes(), ef[:n].tobytes(), st[:n].tobytes())
+    grown = [(int(nsi[r]), nsk[32 * r:32 * r + 32].tobytes()) for r in range(m)]
+    return verdicts, asset_ids, events, (grown, nb[:64 * m].tobytes(), npd[:64 * m].tobytes(), nf[:m].tobytes()), rounds.value
+
+
+def asset_calls_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: int, d_slot_ids_ptr: int, d_slot_keys_ptr: int,
+                              d_balances_ptr: int, d_pendings_ptr: int, d_flags_ptr: int, next_asset_id: int, new_slot_flags: int, n_tx: int,
+                              d_kind_ptr: int, d_asset_id_ptr: int, d_rows_ptr: int, d_proofs_ptr: int, d_verdicts_ptr: int,
+                              d_asset_ids_ptr: int, d_balance_after_ptr: int, d_event_ct_ptr: int, d_event_flags_ptr: int, d_status_ptr: int,
+                              d_new_slot_ids_ptr: int, d_new_slot_keys_ptr: int, d_new_balances_ptr: int, d_new_pendings_ptr: int,
+                              d_new_flags_ptr: int):
+    """zk_import_asset_calls_device on device pointers (d_slot_ids, d_asset_id, d_asset_ids, d_new_slot_ids: uint32; the
+    table outputs with room for n_slots + 2 n_tx rows).  Blocks on the context's stream twice before the rounds and as
+    assets_import_device after; returns (rows of the grown table, rounds), with the outputs complete."""
+    v = lambda x: C.c_void_p(x) if x else None
+    n_out, rounds = C.c_size_t(0), C.c_uint(0)
+    _ck(_lib.lib().zk_import_asset_calls_device(ctx._h, pvk._h, n_slots, v(d_slot_ids_ptr), v(d_slot_keys_ptr), v(d_balances_ptr),
+                                                v(d_pendings_ptr), v(d_flags_ptr), next_asset_id, new_slot_flags & 0xFF, n_tx, v(d_kind_ptr),
+                                                v(d_asset_id_ptr), v(d_rows_ptr), v(d_proofs_ptr), v(d_verdicts_ptr), v(d_asset_ids_ptr),
+                                                v(d_balance_after_ptr), v(d_event_ct_ptr), v(d_event_flags_ptr), v(d_status_ptr),
+                                                v(d_new_slot_ids_ptr), v(d_new_slot_keys_ptr), v(d_new_balances_ptr), v(d_new_pendings_ptr),
+                                                v(d_new_flags_ptr), C.byref(n_out), C.byref(rounds)))
+    return n_out.value, rounds.value
+
+
 def anonymous_import(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
     """import_anonymous_calls_block in one call (zk_import_anonymous_block): the issue rows, both verifications, the verdict
     scatters and both state passes run on the device between one upload and one download, with the proofs checked on
