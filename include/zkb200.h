@@ -44,6 +44,7 @@ extern "C" {
 #define ZK_ERR_DECODE (-7)               /* GroupDecodingError (not on curve, not in subgroup, bad flags, x >= q) */
 #define ZK_ERR_NOT_CANONICAL (-8)        /* a scalar >= r (PrimeFieldDecodingError::NotInField) */
 #define ZK_ERR_MALFORMED_VK (-9)         /* SynthesisError::MalformedVerifyingKey: inputs.len() + 1 != ic.len() */
+#define ZK_ERR_BAD_SIGNATURE (-10)      /* zk_import_block: an extrinsic's signature fails (BadSignature) */
 
 const char *zk_last_error(void);
 int zk_device_count(void);
@@ -604,6 +605,79 @@ int zk_import_anonymous_block_device(zk_ctx *ctx, const zk_pvk *anon_pvk, const 
                                      const uint8_t *d_issue_fields, const uint8_t *d_g_epoch, const uint8_t *d_proofs, uint8_t *d_verdicts,
                                      uint8_t *d_enc_balances, uint8_t *d_issued, uint8_t *d_tx_status, uint8_t *d_new_balances,
                                      uint8_t *d_new_pendings, uint8_t *d_new_flags);
+/* ---- block import: the signatures and all three zk pallets' calls in one call --------------------------------------------
+ * zk_import_block: what Executive::execute_block needs from the zk pallets for one block.  It checks every extrinsic's
+ * signature (the block is rejected if one fails, modules/executive/src/lib.rs:168-183), then imports the block's
+ * confidential transfers, encrypted-asset calls and anonymous-balances calls.  The pallets keep disjoint storage, so
+ * each section's outputs equal, byte for byte, those of its own call on the same arguments:
+ * zk_import_confidential_block, zk_import_asset_calls and zk_import_anonymous_block.  The call shares verifier launches
+ * across sections.  L1 (conf_pvk) verifies the confidential transfers' first round, every asset issue and destroy, and
+ * every anonymous issue.  One launch with anon_pvk verifies the anonymous transfers.  Each later conf_pvk launch verifies
+ * the undecided transfers of both chain-keyed sections: confidential round r with asset round r - 1.  That is
+ * max(R_conf, 1 + R_assets) launches with conf_pvk, R being a section's rounds in its own call, plus one with anon_pvk;
+ * a launch with no proofs is skipped.
+ *
+ * Arguments, in order:
+ *   conf_pvk: the 11-point key of the confidential transfers, the asset calls and the anonymous issues; may be NULL when
+ *     no section has a transaction that uses it.  anon_pvk: the 52-point key; may be NULL when the anonymous section has
+ *     no transaction.  Each key passed must have its shape (ZK_ERR_MALFORMED_VK).
+ *   the signatures: n_sig, vks, sigs, msgs, msg_off, zs exactly as zk_redjubjub_batch_verify takes them (one per
+ *     extrinsic, checked with FixedGenerators::Diversifier).
+ *   c_*: zk_import_confidential_block's arguments less ctx and pvk; a_*: zk_import_asset_calls's less ctx and pvk;
+ *     an_*: zk_import_anonymous_block's less ctx and the keys.  A section with no rows and no transactions is empty
+ *     and needs no pointers beyond what its own call needs at zero size.
+ *   first_bad_sig: the lowest extrinsic whose signature fails, n_sig when none does (may be NULL).
+ *   launches: the verifier launches the call made, with both keys (may be NULL).
+ * Checks, in this order:
+ *   1. NULL arguments and sizes, per section as each call checks them (ZK_ERR_INVALID).
+ *   2. Each section's kinds and indices (ZK_ERR_INVALID; zk_last_error names the section and the lowest transaction or
+ *      table row, e.g. "zk_import_block: assets: transaction 17: ...").
+ *   3. The signatures, as redjubjub_verify_batched: the batch check, then the per-signature verdicts when it fails.
+ *      If any verdict is not 1 the call returns ZK_ERR_BAD_SIGNATURE.  It then verifies no proof and writes no
+ *      output; zk_last_error names the extrinsic and its verdict (0 / 2 / 3 / 4).  Every z_i is checked first: a
+ *      z_i >= r_J gives ZK_ERR_NOT_CANONICAL, naming the lowest such extrinsic.
+ *   4. The proofs and the state passes.  The asset section's id overflow and table size (ZK_ERR_INVALID) and a
+ *      stored ciphertext that does not read (ZK_ERR_DECODE) are reported as each call reports them. */
+int zk_import_block(zk_ctx *ctx, const zk_pvk *conf_pvk, const zk_pvk *anon_pvk, size_t n_sig, const uint8_t *vks, const uint8_t *sigs,
+                    const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *zs, size_t c_n_accounts, const uint8_t *c_balances,
+                    const uint8_t *c_pendings, const uint8_t *c_acct_flags, size_t c_n_tx, const uint32_t *c_sender,
+                    const uint32_t *c_recipient, const uint8_t *c_rows, const uint8_t *c_proofs, uint8_t *c_verdicts,
+                    uint8_t *c_balance_after, uint8_t *c_tx_status, uint8_t *c_new_balances, uint8_t *c_new_pendings, uint8_t *c_new_flags,
+                    unsigned *c_rounds, size_t a_n_slots, const uint32_t *a_slot_ids, const uint8_t *a_slot_keys, const uint8_t *a_balances,
+                    const uint8_t *a_pendings, const uint8_t *a_slot_flags, uint32_t a_next_asset_id, uint8_t a_new_slot_flags,
+                    size_t a_n_tx, const uint8_t *a_kind, const uint32_t *a_asset_id, const uint8_t *a_rows, const uint8_t *a_proofs,
+                    uint8_t *a_verdicts, uint32_t *a_asset_ids, uint8_t *a_balance_after, uint8_t *a_event_ct, uint8_t *a_event_flags,
+                    uint8_t *a_tx_status, uint32_t *a_new_slot_ids, uint8_t *a_new_slot_keys, uint8_t *a_new_balances,
+                    uint8_t *a_new_pendings, uint8_t *a_new_flags, size_t *a_n_slots_out, unsigned *a_rounds, size_t an_n_accounts,
+                    const uint8_t *an_keys, const uint8_t *an_balances, const uint8_t *an_pendings, const uint8_t *an_acct_flags,
+                    size_t an_n_tx, const uint8_t *an_kind, const uint32_t *an_members, const uint8_t *an_tx_points,
+                    const uint8_t *an_tx_extra, const uint8_t *an_issue_fields, const uint8_t *an_g_epoch, const uint8_t *an_proofs,
+                    uint8_t *an_verdicts, uint8_t *an_enc_balances, uint8_t *an_issued, uint8_t *an_tx_status, uint8_t *an_new_balances,
+                    uint8_t *an_new_pendings, uint8_t *an_new_flags, size_t *first_bad_sig, unsigned *launches);
+/* the same with device pointers (the uint32 and uint64 arrays aligned to their size; c_rounds, a_n_slots_out, a_rounds,
+ * first_bad_sig and launches are host pointers; msg_off is not checked and must not decrease).  The call blocks on the
+ * context's stream to read a block of counters: once before L1 (every section's kinds and indices, and the batch
+ * verdict of the signatures), once more when that batch check fails, once after L1 when the confidential transfers
+ * took part in it or the block has an asset section, and once after each later launch.  It returns with the outputs complete. */
+int zk_import_block_device(zk_ctx *ctx, const zk_pvk *conf_pvk, const zk_pvk *anon_pvk, size_t n_sig, const uint8_t *d_vks,
+                           const uint8_t *d_sigs, const uint8_t *d_msgs, const uint64_t *d_msg_off, const uint8_t *d_zs, size_t c_n_accounts,
+                           const uint8_t *d_c_balances, const uint8_t *d_c_pendings, const uint8_t *d_c_acct_flags, size_t c_n_tx,
+                           const uint32_t *d_c_sender, const uint32_t *d_c_recipient, const uint8_t *d_c_rows, const uint8_t *d_c_proofs,
+                           uint8_t *d_c_verdicts, uint8_t *d_c_balance_after, uint8_t *d_c_tx_status, uint8_t *d_c_new_balances,
+                           uint8_t *d_c_new_pendings, uint8_t *d_c_new_flags, unsigned *c_rounds, size_t a_n_slots,
+                           const uint32_t *d_a_slot_ids, const uint8_t *d_a_slot_keys, const uint8_t *d_a_balances,
+                           const uint8_t *d_a_pendings, const uint8_t *d_a_slot_flags, uint32_t a_next_asset_id, uint8_t a_new_slot_flags,
+                           size_t a_n_tx, const uint8_t *d_a_kind, const uint32_t *d_a_asset_id, const uint8_t *d_a_rows,
+                           const uint8_t *d_a_proofs, uint8_t *d_a_verdicts, uint32_t *d_a_asset_ids, uint8_t *d_a_balance_after,
+                           uint8_t *d_a_event_ct, uint8_t *d_a_event_flags, uint8_t *d_a_tx_status, uint32_t *d_a_new_slot_ids,
+                           uint8_t *d_a_new_slot_keys, uint8_t *d_a_new_balances, uint8_t *d_a_new_pendings, uint8_t *d_a_new_flags,
+                           size_t *a_n_slots_out, unsigned *a_rounds, size_t an_n_accounts, const uint8_t *d_an_keys,
+                           const uint8_t *d_an_balances, const uint8_t *d_an_pendings, const uint8_t *d_an_acct_flags, size_t an_n_tx,
+                           const uint8_t *d_an_kind, const uint32_t *d_an_members, const uint8_t *d_an_tx_points,
+                           const uint8_t *d_an_tx_extra, const uint8_t *d_an_issue_fields, const uint8_t *d_an_g_epoch,
+                           const uint8_t *d_an_proofs, uint8_t *d_an_verdicts, uint8_t *d_an_enc_balances, uint8_t *d_an_issued,
+                           uint8_t *d_an_tx_status, uint8_t *d_an_new_balances, uint8_t *d_an_new_pendings, uint8_t *d_an_new_flags,
+                           size_t *first_bad_sig, unsigned *launches);
 /* Engine::pairing (core/pairing/src/lib.rs:108-115, bls12_381/mod.rs:40-160) for n pairs of checked G1Uncompressed /
  * G2Uncompressed encodings; out: n * 576 bytes in Fq12::write order (fq12.rs:29-45). */
 int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const uint8_t *g2, uint8_t *out);

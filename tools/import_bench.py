@@ -23,6 +23,14 @@
     anonymous_import (zk_import_anonymous_block), and the two verify_proofs_with_points_device launches alone (issues on
     11 points, transfers on 52) on device-resident rows.  Proofs are forged from toy keys of the real shapes' input counts
     (tests/import_anon_corpus.py); the outputs are checked against anon_issue_coracle.c.
+  - with --block, instead of the three legs above, one block of all three (the same sizes, one signature per
+    transaction: 256 distinct signatures tiled, z_i drawn once before the reps), three arms alternated:
+      block    block_import (zk_import_block: the signatures, then every section on one schedule of shared launches)
+      calls    the four calls in sequence: redjubjub_verify_batched, confidential_import, asset_calls_import,
+               anonymous_import
+      verify   one 11-point verify_proofs_with_points_device launch over every confidential, asset and anonymous-issue
+               proof and one 52-point launch over the anonymous transfers, on device-resident rows
+    and the verifier launches each import arm makes.  Every output is checked against the others and the C oracles.
 A leg with 0 transactions is skipped.
 --fail-rate is the fraction of transfers (and of issues and destroys) whose proof fails; a transfer after a failure in its
 chain is proven against the balance without it, so each failure costs a round.  Proofs are forged from a toy key's
@@ -82,6 +90,7 @@ def main():
     ap.add_argument("--skew", type=float, default=1.0)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--seed", type=int, default=7)
+    ap.add_argument("--block", action="store_true", help="the whole-block leg instead of the three pallet legs")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -106,9 +115,9 @@ def main():
             return d_out.cpu().numpy().tobytes()
         return run
 
-    def measure(label, driver, call, verify, check, extra=()):
+    def measure(label, driver, call, verify, check, extra=(), names=("driver", "call")):
         """the arms driver, call, verify and any (name, fn) in extra, alternated; name_over_verify for every arm"""
-        arms = [("driver", driver), ("call", call), ("verify", verify)] + list(extra)
+        arms = [(names[0], driver), (names[1], call), ("verify", verify)] + list(extra)
         for _, fn in arms:                           # warm-up: module loads, workspace growth
             fn()
         times = {k: [] for k, _ in arms}
@@ -123,11 +132,13 @@ def main():
         res.update({"%s_over_verify" % k: round(med[k] / med["verify"], 3) for k, _ in arms if k != "verify"})
         return res
 
-    if a.conf_tx:
+    if a.block:
+        res["block"] = block_leg(a, ctx, measure)
+    if a.conf_tx and not a.block:
         res["confidential"] = confidential_leg(a, ctx, key, pvk, measure, verify_alone)
-    if a.asset_tx:
+    if a.asset_tx and not a.block:
         res["assets"] = assets_leg(a, ctx, key, pvk, measure, verify_alone)
-    if a.anon_tx:
+    if a.anon_tx and not a.block:
         res["anonymous"] = anonymous_leg(a, ctx, measure)
     res["outputs_equal_oracle"] = True
     pvk.free()
@@ -276,6 +287,77 @@ def anonymous_leg(a, ctx, measure):
              n_tx=a.anon_tx, accounts=a.accounts, issues=len(iss), failures=sum(v != 1 for v in want[0]))
     apvk.free()
     cpvk.free()
+    return r
+
+
+def block_leg(a, ctx, measure):
+    import torch
+    from tests.jubjub_oracle import redjubjub as rj
+    conf, anon = iac.ForgeKey(zk.CONFIDENTIAL_POINTS, 171), iac.ForgeKey(zk.ANONYMOUS_POINTS, 71)
+    cpvk, apvk = zk.PreparedVerifyingKey.prepare(ctx, conf.params_bytes), zk.PreparedVerifyingKey.prepare(ctx, anon.params_bytes)
+    log("block corpus: %d confidential, %d asset, %d anonymous calls" % (a.conf_tx, a.asset_tx, a.anon_tx))
+    cb = ic.confidential(conf, a.accounts, a.conf_tx, a.seed, fail_frac=a.fail_rate, skew=a.skew)
+    ab = ic.assets(conf, a.slots, a.asset_tx, a.seed + 1, fail_frac=a.fail_rate, fixed_fail_frac=a.fail_rate, issue_frac=a.issue_frac,
+                   destroy_frac=a.destroy_frac, skew=a.skew, state_call=lambda *x: zk.assets_block(ctx, *x))
+    nb = iac.block(anon, conf, a.accounts, a.anon_tx, a.seed + 2, issue_frac=a.issue_frac, fail_frac=a.fail_rate, skew=a.skew)
+    n_sig = a.conf_tx + a.asset_tx + a.anon_tx
+    distinct = []
+    for i in range(256):
+        sk = rj.spending_key(b"bench-%d" % i)
+        msg = b"extrinsic %d" % i
+        distinct.append((rj.public_key(sk), rj.sign(sk, msg, bytes([i]) * 80), msg))
+    vks, sigs, msgs = ([distinct[i % 256][j] for i in range(n_sig)] for j in range(3))
+    sig = (vks, sigs, msgs, zk.random_batch_scalars(n_sig))    # drawn once: neither arm times the draw
+    c_args, a_args, n_args = (cb.accounts, cb.txs, cb.proofs), ab.args(), nb.args()
+    want = (zk.confidential_import(ctx, cpvk, *c_args), zk.asset_calls_import(ctx, cpvk, *a_args), zk.anonymous_import(ctx, apvk, cpvk, *n_args))
+    log("C oracles (block)")
+    assert [w[0] for w in want] == [cb.intended, ab.intended, nb.intended], "verdicts differ from the intended ones"
+    co, ao, no = cb.oracle(want[0][0]), ab.oracle(want[1][0]), nb.oracle(want[2][0])
+    assert want[0][2] == co[0] and want[0][1] == tuple(co[2:]), "the confidential import differs from the C oracle"
+    assert want[1][3][1:] == ao[5:], "the asset import differs from the C oracle"
+    assert want[2][2] == no[0] and want[2][1] == no[4:], "the anonymous import differs from the C oracle"
+    iss = [k for k, t in enumerate(nb.txs) if t.kind == zk.ANON_ISSUE]
+    tr = [k for k, t in enumerate(nb.txs) if t.kind == zk.ANON_TRANSFER]
+    dev = torch.device("cuda", 0)
+    up = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev) if b else torch.zeros(1, dtype=torch.uint8, device=dev)
+    rows11 = cb.rows + ab.rows + b"".join(nb.txs[k].verify_points(nb.accounts[0], nb.g_epoch) for k in iss)
+    proofs11 = b"".join(cb.proofs) + b"".join(ab.proofs) + b"".join(nb.proofs[k] for k in iss)
+    n11 = len(proofs11) // 192
+    d_r11, d_p11 = up(rows11), up(proofs11)
+    d_r52, d_p52 = up(b"".join(no[1][1664 * k:1664 * k + 1664] for k in tr)), up(b"".join(nb.proofs[k] for k in tr))
+    d_out = torch.zeros(n11 + len(tr) + 1, dtype=torch.uint8, device=dev)
+    v_want = bytes(cb.intended + ab.intended + [nb.intended[k] for k in iss + tr])
+    torch.cuda.synchronize()
+
+    def verify():
+        zk.verify_proofs_with_points_device(cpvk, n11, d_p11.data_ptr(), d_r11.data_ptr(), zk.CONFIDENTIAL_POINTS, d_out.data_ptr())
+        if tr:
+            zk.verify_proofs_with_points_device(apvk, len(tr), d_p52.data_ptr(), d_r52.data_ptr(), zk.ANONYMOUS_POINTS,
+                                                d_out.data_ptr() + n11)
+        ctx.sync()
+        return d_out[:n11 + len(tr)].cpu().numpy().tobytes()
+
+    launches = {}
+
+    def block():
+        r = zk.block_import(ctx, cpvk, apvk, sig, c_args, a_args, n_args)
+        launches["block"] = r.launches
+        return r[:3]
+
+    def calls():
+        assert zk.redjubjub_verify_batched(ctx, *sig) == [zk.REDJUBJUB_OK] * n_sig
+        out = (zk.confidential_import(ctx, cpvk, *c_args), zk.asset_calls_import(ctx, cpvk, *a_args),
+               zk.anonymous_import(ctx, apvk, cpvk, *n_args))
+        launches["calls"] = (out[0][3] + out[1][4] + any(t.kind != zk.ASSET_TRANSFER for t in ab.txs) + (len(iss) > 0) + (len(tr) > 0))
+        return out
+
+    def check(k, out):
+        assert out == (v_want if k == "verify" else want), "%s differs" % k
+    r = dict(measure("block", calls, block, verify, check, names=("calls", "block")), signatures=n_sig,
+             failures=sum(v != 1 for w in want for v in w[0]), rounds={"confidential": want[0][3], "assets": want[1][4]})
+    r["launches"] = launches
+    cpvk.free()
+    apvk.free()
     return r
 
 

@@ -93,6 +93,12 @@ SIGNATURES = {
     "zk_import_asset_calls_device": (i32, [vp, vp, sz] + [vp] * 5 + [u32, C.c_uint8, sz] + [vp] * 15 + [C.POINTER(sz), C.POINTER(u32)]),
     "zk_import_anonymous_block": (i32, [vp, vp, vp, sz, vp, vp, vp, vp, sz] + [vp] * 14),
     "zk_import_anonymous_block_device": (i32, [vp, vp, vp, sz, vp, vp, vp, vp, sz] + [vp] * 14),
+    "zk_import_block": (i32, [vp, vp, vp, sz, vp, vp, vp, vp, vp] + [sz, vp, vp, vp, sz] + [vp] * 10 + [C.POINTER(u32)] + [sz] + [vp] * 5 +
+                        [u32, C.c_uint8, sz] + [vp] * 15 + [C.POINTER(sz), C.POINTER(u32)] + [sz, vp, vp, vp, vp, sz] + [vp] * 14 +
+                        [C.POINTER(sz), C.POINTER(u32)]),
+    "zk_import_block_device": (i32, [vp, vp, vp, sz, vp, vp, vp, vp, vp] + [sz, vp, vp, vp, sz] + [vp] * 10 + [C.POINTER(u32)] + [sz] +
+                               [vp] * 5 + [u32, C.c_uint8, sz] + [vp] * 15 + [C.POINTER(sz), C.POINTER(u32)] + [sz, vp, vp, vp, vp, sz] +
+                               [vp] * 14 + [C.POINTER(sz), C.POINTER(u32)]),
     "zk_pairing_batch": (i32, [vp, sz, vp, vp, vp]),
 }
 
@@ -118,6 +124,9 @@ def lib():
             fn.argtypes = args
         _lib = L
     return _lib
+
+
+ZK_ERR_BAD_SIGNATURE = -10     # zk_import_block: an extrinsic's signature fails
 
 
 def check(code):

@@ -23,7 +23,7 @@
 //   4. imp_an_gather: each transfer's 52 points from that pass and its proof, verified with the anonymous key,
 //   5. imp_an_scatter: the transfer verdicts, then the state pass again.
 // zk_import_asset_calls (section 6) puts the asset numbering and the slot resolution in front of zk_import_assets_block's
-// rounds.
+// rounds.  zk_import_block (section 7) runs the sections of all three pallets on one schedule, sharing the launches.
 //
 // Plain integer code, one function per item and thread of each pass; the same source compiles with ZK_HOST_EMUL for the
 // CPU tests (tests/host_emul/emul_import.cpp, emul_import_anon.cpp, emul_import_assets.cpp), which run the passes as loops
@@ -101,15 +101,16 @@ ZK_IMP_DEV bool imp_undecided(size_t k, const uint8_t *kind, const uint8_t *verd
 ZK_IMP_DEV void imp_flag(size_t k, const uint8_t *kind, const uint8_t *verdict, uint32_t *flag) { flag[k] = imp_undecided(k, kind, verdict); }
 
 // Item i: word w = i % IMP_WORDS of transaction k = i / IMP_WORDS, when k is undecided: words [0, 88) are its verifier
-// row, with bytes [192, 256) taken from balance_sender[k], words [88, 136) its proof.  Word 0 also records k as the row's
-// transaction.  Byte copies: the caller's arrays need no alignment.
+// row, with bytes [192, 256) taken from balance_sender[k], words [88, 136) its proof, into row off + pos[k] of the round
+// buffers (off: the section's first row in a launch shared with other sections).  Word 0 also records k as the
+// section's row pos[k].  Byte copies: the caller's arrays need no alignment.
 ZK_IMP_DEV void imp_gather(size_t i, const uint8_t *kind, const uint8_t *verdict, const uint32_t *pos, const uint8_t *rows, const uint8_t *proofs,
-                           const uint8_t *balance_sender, uint32_t *idx, uint8_t *round_rows, uint8_t *round_proofs) {
+                           const uint8_t *balance_sender, uint32_t *idx, uint8_t *round_rows, uint8_t *round_proofs, size_t off = 0) {
     const size_t k = i / IMP_WORDS;
     const uint32_t w = (uint32_t)(i % IMP_WORDS);
     if (!imp_undecided(k, kind, verdict)) return;
-    const size_t j = pos[k];
-    if (!w) idx[j] = (uint32_t)k;
+    if (!w) idx[pos[k]] = (uint32_t)k;
+    const size_t j = off + pos[k];
     const uint32_t o = 4 * w;
     const uint8_t *src;
     uint8_t *dst;
@@ -136,10 +137,11 @@ ZK_IMP_DEV void imp_tx_points(size_t i, const uint8_t *rows, uint8_t *tx_points)
 }
 
 // ---- 4. decisions ------------------------------------------------------------------------------------------------------
-// row j of m: transaction idx[j] with verdict rv[j].  A failure lowers its chain's first_fail (IMP_NONE before the pass)
-// and counts in cnt[IMP_FAILS].
-ZK_IMP_DEV void imp_fail(size_t j, const uint32_t *idx, const uint32_t *key_a, const uint8_t *rv, uint32_t *first_fail, uint32_t *cnt) {
-    if (rv[j] == 1) return;
+// row j of the section's m: transaction idx[j] with verdict rv[off + j].  A failure lowers its chain's first_fail
+// (IMP_NONE before the pass) and counts in cnt[IMP_FAILS].
+ZK_IMP_DEV void imp_fail(size_t j, const uint32_t *idx, const uint32_t *key_a, const uint8_t *rv, uint32_t *first_fail, uint32_t *cnt,
+                         size_t off = 0) {
+    if (rv[off + j] == 1) return;
     const uint32_t k = idx[j];
     imp_min(first_fail + key_a[k], k);
     imp_inc(cnt + IMP_FAILS);
@@ -147,11 +149,11 @@ ZK_IMP_DEV void imp_fail(size_t j, const uint32_t *idx, const uint32_t *key_a, c
 // after every imp_fail: a transaction at or before its chain's first failure takes its verdict, and is applied iff it
 // passed; one after it stays undecided and applied, and counts in cnt[IMP_LEFT]
 ZK_IMP_DEV void imp_decide(size_t j, const uint32_t *idx, const uint32_t *key_a, const uint8_t *rv, const uint32_t *first_fail,
-                           uint8_t *verdict, uint8_t *applied, uint32_t *cnt) {
+                           uint8_t *verdict, uint8_t *applied, uint32_t *cnt, size_t off = 0) {
     const uint32_t k = idx[j];
     if (k <= first_fail[key_a[k]]) {
-        verdict[k] = rv[j];
-        applied[k] = rv[j] == 1;
+        verdict[k] = rv[off + j];
+        applied[k] = rv[off + j] == 1;
     } else {
         imp_inc(cnt + IMP_LEFT);
     }
@@ -190,14 +192,14 @@ ZK_IMP_DEV void imp_an_start(size_t k, uint32_t n_acct, bool issues_ok, const ui
 // Item i: word w = i % IMP_AN_ISSUE_WORDS of transaction k = i / IMP_AN_ISSUE_WORDS, when k is an issue; pos[k] is its row.
 // Words [0, 88) are verify_confidential_proof's 11 points over (issuer, issuer, total, total, randomness, fee, balance, rvk,
 // g_epoch, nonce): keys[issuer], tx_points slots 0 and 12, issue_fields (fee | balance), tx_extra (rvk | nonce) and g_epoch.
-// Words [88, 136) are its proof.  Byte copies: the caller's arrays need no alignment.
+// Words [88, 136) are its proof.  Both go to row off + pos[k].  Byte copies: the caller's arrays need no alignment.
 ZK_IMP_DEV void imp_an_issue_row(size_t i, const uint8_t *kind, const uint32_t *pos, const uint8_t *keys, const uint32_t *members,
                                  const uint8_t *tx_points, const uint8_t *issue_fields, const uint8_t *tx_extra, const uint8_t *g_epoch,
-                                 const uint8_t *proofs, uint8_t *rows, uint8_t *round_proofs) {
+                                 const uint8_t *proofs, uint8_t *rows, uint8_t *round_proofs, size_t off = 0) {
     const size_t k = i / IMP_AN_ISSUE_WORDS;
     const uint32_t o = 4 * (uint32_t)(i % IMP_AN_ISSUE_WORDS);
     if (kind[k] != IMP_AN_ISSUE) return;
-    const size_t j = pos[k];
+    const size_t j = off + pos[k];
     const uint8_t *src;
     uint8_t *dst;
     if (o < IMP_ROW) {
@@ -223,25 +225,26 @@ ZK_IMP_DEV void imp_an_issue_row(size_t i, const uint8_t *kind, const uint32_t *
 
 // pos is the exclusive prefix sum of the flags "not a transfer" (an anonymous issue; an asset issue or destroy), so
 // pos[k] is such a transaction's compact row and k - pos[k] a transfer's.
-// issues: verdicts[k] = rv[pos[k]] at a non-transfer and 0 at a transfer (not applied in the first state pass); otherwise
-// verdicts[k] = rv[k - pos[k]] at a transfer, the others unchanged.
-ZK_IMP_DEV void imp_an_scatter(size_t k, bool issues, const uint8_t *kind, const uint32_t *pos, const uint8_t *rv, uint8_t *verdicts) {
+// issues: verdicts[k] = rv[off + pos[k]] at a non-transfer and 0 at a transfer (not applied in the first state pass);
+// otherwise verdicts[k] = rv[off + k - pos[k]] at a transfer, the others unchanged.
+ZK_IMP_DEV void imp_an_scatter(size_t k, bool issues, const uint8_t *kind, const uint32_t *pos, const uint8_t *rv, uint8_t *verdicts,
+                               size_t off = 0) {
     const bool issue = kind[k] != IMP_AN_TRANSFER;
     if (issues)
-        verdicts[k] = issue ? rv[pos[k]] : 0;
+        verdicts[k] = issue ? rv[off + pos[k]] : 0;
     else if (!issue)
-        verdicts[k] = rv[k - pos[k]];
+        verdicts[k] = rv[off + k - pos[k]];
 }
 
 // Item i: word o / 4 of transaction k's row_bytes-byte row (src_rows) and 192-byte proof, when k is a non-transfer (issues)
-// or a transfer (!issues): into compact row pos[k] or k - pos[k] of rows / round_proofs.
+// or a transfer (!issues): into compact row off + pos[k] or off + k - pos[k] of rows / round_proofs.
 ZK_IMP_DEV void imp_compact(size_t i, uint32_t row_bytes, bool issues, const uint8_t *kind, const uint32_t *pos, const uint8_t *src_rows,
-                            const uint8_t *proofs, uint8_t *rows, uint8_t *round_proofs) {
+                            const uint8_t *proofs, uint8_t *rows, uint8_t *round_proofs, size_t off = 0) {
     const uint32_t words = (row_bytes + 192) / 4;
     const size_t k = i / words;
     const uint32_t o = 4 * (uint32_t)(i % words);
     if ((kind[k] != IMP_AN_TRANSFER) != issues) return;
-    const size_t j = issues ? pos[k] : k - pos[k];
+    const size_t j = off + (issues ? pos[k] : k - pos[k]);
     const uint8_t *src;
     uint8_t *dst;
     if (o < row_bytes) {
@@ -434,6 +437,38 @@ ZK_IMP_DEV void imp_as_tx_points(size_t i, const uint8_t *kind, const uint8_t *r
     }
 #pragma unroll
     for (int b = 0; b < 4; b++) tx_points[4 * i + b] = 0;
+}
+
+// ---- 7. zk_import_block -----------------------------------------------------------------------------------------------
+// One launch verifies the rows of several sections (the confidential transfers, the asset calls, the anonymous issues)
+// that use one key: each section compacts its rows behind the ones before it (imp_gather / imp_compact / imp_an_issue_row
+// with off, the rows of the sections before it), the verifier runs once over them all, and each section reads its
+// verdicts at its own offset (imp_fail / imp_decide / imp_an_scatter with off), over its own chain keys.  A section's
+// rows are a contiguous run of the launch, so no verdict of one section is read by another.
+// the lowest extrinsic whose signature verdict is not 1 into *first (IMP_NONE before the pass)
+ZK_IMP_DEV void imp_sig_first(size_t i, const uint8_t *verdicts, uint32_t *first) {
+    if (verdicts[i] != 1) imp_min(first, (uint32_t)i);
+}
+// after imp_sig_first: that extrinsic's verdict into *code (1 when every signature passes)
+ZK_IMP_DEV void imp_sig_code(const uint8_t *verdicts, const uint32_t *first, uint32_t *code) {
+    *code = *first != IMP_NONE ? verdicts[*first] : 1;
+}
+// a 32-byte little-endian z below r_J?  Every z is checked before the batch verdict is read, as zk_redjubjub_batch_verify
+// checks them before it computes anything.
+ZK_IMP_DEV bool imp_fs_canonical(const uint8_t *b) {
+    const uint64_t r[4] = {0xd0970e5ed6f72cb7ull, 0xa6682093ccc81082ull, 0x06673b0101343b00ull, 0x0e7db4ea6533afa9ull};
+#pragma unroll
+    for (int w = 3; w >= 0; w--) {
+        uint64_t v = 0;
+#pragma unroll
+        for (int k = 7; k >= 0; k--) v = v << 8 | b[8 * w + k];
+        if (v != r[w]) return v < r[w];
+    }
+    return false;
+}
+// the lowest extrinsic whose z_i >= r_J into *first (IMP_NONE before the pass)
+ZK_IMP_DEV void imp_sig_z(size_t i, const uint8_t *zs, uint32_t *first) {
+    if (!imp_fs_canonical(zs + 32 * i)) imp_min(first, (uint32_t)i);
 }
 
 }  // namespace zkimp

@@ -14,7 +14,9 @@ importing works without a GPU, any compute call without one raises ZkError(ZK_ER
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
+import re
 import secrets
 
 import numpy as np
@@ -1141,14 +1143,12 @@ def _confidential_rows(txs) -> bytes:
                     bytes(64) + t.rvk + t.g_epoch + t.nonce for t in txs)
 
 
-def confidential_import(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, proofs):
-    """import_confidential_block in one call (zk_import_confidential_block): the rounds run on the device, between one
-    upload and one download, and the proofs are checked on ctx.  Same arguments, result and errors, except that a key of
-    another shape raises SynthesisError(MalformedVerifyingKey) even for a block without transfers."""
+def _conf_section(name: str, accounts, txs, proofs):
+    """confidential_import's C arguments after ctx and the key, and the function that reads its result from them"""
     balances, pendings, flags = accounts
     n_acct, n = len(flags), len(txs)
     if any(not (0 <= t.sender < 2**32 and 0 <= t.recipient < 2**32) for t in txs):
-        raise ValueError("confidential_import: account index out of range")
+        raise ValueError("%s: account index out of range" % name)
     proofs = _cat(proofs, 192)
     bal, pend, fl = _cat(balances, 64), _cat(pendings, 64), bytes(flags)
     assert len(proofs) == 192 * n and len(bal) == len(pend) == 64 * n_acct
@@ -1157,17 +1157,28 @@ def confidential_import(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, 
     z = lambda m: np.zeros(max(m, 1), np.uint8)
     v, ba, st, nb, npd, nf = z(n), z(64 * n), z(n), z(64 * n_acct), z(64 * n_acct), z(n_acct)
     rounds = C.c_uint(0)
+    keep = [buf(bal), buf(pend), buf(fl), idx([t.sender for t in txs]), idx([t.recipient for t in txs]), buf(_confidential_rows(txs)),
+            buf(proofs)]
+    args = [n_acct] + [_p(a) for a in keep[:3]] + [n] + [_p(a) for a in keep[3:]] + [_p(x) for x in (v, ba, st, nb, npd, nf)] + [C.byref(rounds)]
+
+    def result():
+        return ([int(x) for x in v[:n]], (nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes()),
+                ba[:64 * n].tobytes(), rounds.value)
+    return args, result, keep
+
+
+def confidential_import(ctx: Context, pvk: PreparedVerifyingKey, accounts, txs, proofs):
+    """import_confidential_block in one call (zk_import_confidential_block): the rounds run on the device, between one
+    upload and one download, and the proofs are checked on ctx.  Same arguments, result and errors, except that a key of
+    another shape raises SynthesisError(MalformedVerifyingKey) even for a block without transfers."""
+    args, result, _keep = _conf_section("confidential_import", accounts, txs, proofs)
     if pvk.ctx is not ctx:
         pvk.ctx.sync()
     try:
-        _ck(_lib.lib().zk_import_confidential_block(ctx._h, pvk._h, n_acct, _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n,
-                                                    _p(idx([t.sender for t in txs])), _p(idx([t.recipient for t in txs])),
-                                                    _p(buf(_confidential_rows(txs))), _p(buf(proofs)), _p(v), _p(ba), _p(st), _p(nb), _p(npd),
-                                                    _p(nf), C.byref(rounds)))
+        _ck(_lib.lib().zk_import_confidential_block(ctx._h, pvk._h, *args))
     except ZkError as e:
         raise _import_error("confidential_import", e) from None
-    return ([int(x) for x in v[:n]], (nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes()),
-            ba[:64 * n].tobytes(), rounds.value)
+    return result()
 
 
 def confidential_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_accounts: int, d_balances_ptr: int, d_pendings_ptr: int,
@@ -1245,11 +1256,8 @@ def assets_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: int, 
     return rounds.value
 
 
-def asset_calls_import(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
-    """import_assets_block in one call (zk_import_asset_calls): the issue and destroy verification, the asset numbering, the
-    slot resolution and the transfer rounds all run on the device between one upload and one download, with the proofs
-    checked on ctx.  Same arguments, result and errors, plus a ValueError for a slot table that holds one (asset id, key)
-    twice; a key of another shape raises as confidential_import does.  Asset ids (and next_asset_id) are AssetId = u32."""
+def _asset_section(name: str, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
+    """asset_calls_import's C arguments after ctx and the key, and the function that reads its result from them"""
     slots, balances, pendings, flags = state
     slots = [(int(a), _pt32(k)) for a, k in slots]
     n, ns = len(txs), len(slots)
@@ -1257,7 +1265,7 @@ def asset_calls_import(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proo
     assert len(proofs) == 192 * n and len(flags) == ns
     ids = [a for a, _ in slots] + [t.asset_id for t in txs if t.kind != ASSET_ISSUE] + [int(next_asset_id)]
     if any(not 0 <= a <= ASSET_ID_MAX for a in ids):
-        raise ValueError("asset_calls_import: asset id out of range")
+        raise ValueError("%s: asset id out of range" % name)
     rows = b"".join(t.verify_points(bytes(64)) if t.kind == ASSET_TRANSFER else t.verify_points() for t in txs)
     buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
     u32 = lambda a: np.array(a or [0], np.uint32)
@@ -1266,26 +1274,43 @@ def asset_calls_import(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proo
     v, aid, ba, ev, ef, st = z(n), u32([0] * n), z(64 * n), z(128 * n), z(n), z(n)
     nsi, nsk, nb, npd, nf = u32([0] * nr), z(32 * nr), z(64 * nr), z(64 * nr), z(nr)
     n_out, rounds = C.c_size_t(0), C.c_uint(0)
+    keep = [u32([a for a, _ in slots]), buf(b"".join(k for _, k in slots)), buf(_cat(balances, 64)), buf(_cat(pendings, 64)),
+            buf(bytes(flags)), buf(bytes(t.kind for t in txs)), u32([t.asset_id if t.kind != ASSET_ISSUE else 0 for t in txs]), buf(rows),
+            buf(proofs)]
+    args = ([ns] + [_p(a) for a in keep[:5]] + [int(next_asset_id), new_slot_flags & 0xFF, n] + [_p(a) for a in keep[5:]] +
+            [_p(x) for x in (v, aid, ba, ev, ef, st, nsi, nsk, nb, npd, nf)] + [C.byref(n_out), C.byref(rounds)])
+
+    def result():
+        m = n_out.value
+        kinds = bytes(t.kind for t in txs)
+        verdicts = [int(x) for x in v[:n]]
+        asset_ids = [int(aid[k]) if kinds[k] == ASSET_ISSUE and verdicts[k] == 1 else None for k in range(n)]
+        events = _asset_events(kinds, ba[:64 * n].tobytes(), ev[:128 * n].tobytes(), ef[:n].tobytes(), st[:n].tobytes())
+        grown = [(int(nsi[r]), nsk[32 * r:32 * r + 32].tobytes()) for r in range(m)]
+        return verdicts, asset_ids, events, (grown, nb[:64 * m].tobytes(), npd[:64 * m].tobytes(), nf[:m].tobytes()), rounds.value
+    return args, result, keep
+
+
+def _asset_error(name: str, e: ZkError):
+    """zk_import_asset_calls's ZK_ERR_INVALID for an id overflow or a repeated table row becomes a ValueError"""
+    if e.code == -2 and ("2^32 - 1" in str(e) or "repeats" in str(e)):
+        return ValueError("%s: %s" % (name, e))
+    return e
+
+
+def asset_calls_import(ctx: Context, pvk: PreparedVerifyingKey, state, txs, proofs, next_asset_id: int, new_slot_flags: int):
+    """import_assets_block in one call (zk_import_asset_calls): the issue and destroy verification, the asset numbering, the
+    slot resolution and the transfer rounds all run on the device between one upload and one download, with the proofs
+    checked on ctx.  Same arguments, result and errors, plus a ValueError for a slot table that holds one (asset id, key)
+    twice; a key of another shape raises as confidential_import does.  Asset ids (and next_asset_id) are AssetId = u32."""
+    args, result, _keep = _asset_section("asset_calls_import", state, txs, proofs, next_asset_id, new_slot_flags)
     if pvk.ctx is not ctx:
         pvk.ctx.sync()
     try:
-        _ck(_lib.lib().zk_import_asset_calls(ctx._h, pvk._h, ns, _p(u32([a for a, _ in slots])), _p(buf(b"".join(k for _, k in slots))),
-                                             _p(buf(_cat(balances, 64))), _p(buf(_cat(pendings, 64))), _p(buf(bytes(flags))),
-                                             int(next_asset_id), new_slot_flags & 0xFF, n, _p(buf(bytes(t.kind for t in txs))),
-                                             _p(u32([t.asset_id if t.kind != ASSET_ISSUE else 0 for t in txs])), _p(buf(rows)),
-                                             _p(buf(proofs)), _p(v), _p(aid), _p(ba), _p(ev), _p(ef), _p(st), _p(nsi), _p(nsk), _p(nb),
-                                             _p(npd), _p(nf), C.byref(n_out), C.byref(rounds)))
+        _ck(_lib.lib().zk_import_asset_calls(ctx._h, pvk._h, *args))
     except ZkError as e:
-        if e.code == -2 and ("2^32 - 1" in str(e) or "repeats" in str(e)):
-            raise ValueError("asset_calls_import: %s" % e) from None
-        raise
-    m = n_out.value
-    kinds = bytes(t.kind for t in txs)
-    verdicts = [int(x) for x in v[:n]]
-    asset_ids = [int(aid[k]) if kinds[k] == ASSET_ISSUE and verdicts[k] == 1 else None for k in range(n)]
-    events = _asset_events(kinds, ba[:64 * n].tobytes(), ev[:128 * n].tobytes(), ef[:n].tobytes(), st[:n].tobytes())
-    grown = [(int(nsi[r]), nsk[32 * r:32 * r + 32].tobytes()) for r in range(m)]
-    return verdicts, asset_ids, events, (grown, nb[:64 * m].tobytes(), npd[:64 * m].tobytes(), nf[:m].tobytes()), rounds.value
+        raise _asset_error("asset_calls_import", e) from None
+    return result()
 
 
 def asset_calls_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: int, d_slot_ids_ptr: int, d_slot_keys_ptr: int,
@@ -1308,15 +1333,12 @@ def asset_calls_import_device(ctx: Context, pvk: PreparedVerifyingKey, n_slots: 
     return n_out.value, rounds.value
 
 
-def anonymous_import(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
-    """import_anonymous_calls_block in one call (zk_import_anonymous_block): the issue rows, both verifications, the verdict
-    scatters and both state passes run on the device between one upload and one download, with the proofs checked on
-    ctx.  Same arguments, result and errors (conf_pvk may be None when the block has no issue), except that a key of
-    another shape raises SynthesisError(MalformedVerifyingKey) even when the block does not use it."""
+def _anon_section(name: str, accounts, txs, g_epoch, proofs):
+    """anonymous_import's C arguments after ctx and the keys, and the function that reads its result from them"""
     keys, balances, pendings, flags = accounts
     n_acct, n = len(flags), len(txs)
     if any(not all(0 <= m < 2**32 for m in t.members) for t in txs):
-        raise ValueError("anonymous_import: account index out of range")
+        raise ValueError("%s: account index out of range" % name)
     proofs = _cat(proofs, 192)
     ky, bal, pend, fl, ge = _cat(keys, 32), _cat(balances, 64), _cat(pendings, 64), bytes(flags), _pt32(g_epoch)
     assert len(proofs) == 192 * n and len(ky) == 32 * n_acct and len(bal) == len(pend) == 64 * n_acct
@@ -1328,20 +1350,32 @@ def anonymous_import(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: Pre
     mem = np.array([t.members for t in txs] or [[0]], np.uint32).reshape(-1)
     v, eb, iss, st = z(n), z(64 * ANONIMITY_SIZE * n), z(64 * n), z(n)
     nb, npd, nf = z(64 * n_acct), z(64 * n_acct), z(n_acct)
+    keep = [buf(ky), buf(bal), buf(pend), buf(fl), buf(kind), mem, buf(b"".join(t.points() for t in txs)),
+            buf(b"".join(t.rvk + t.nonce for t in txs)), buf(fields), buf(ge), buf(proofs)]
+    args = ([n_acct] + [_p(a) for a in keep[:4]] + [n] + [_p(a) for a in keep[4:8]] + [_p(keep[8]) if has_issue else None] +
+            [_p(a) for a in keep[9:]] + [_p(x) for x in (v, eb, iss, st, nb, npd, nf)])
+
+    def result():
+        issued = [iss[64 * k:64 * k + 64].tobytes() if kind[k] == ANON_ISSUE and st[k] == BLOCK_APPLIED else None for k in range(n)]
+        return ([int(x) for x in v[:n]], (nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes()),
+                eb[:64 * ANONIMITY_SIZE * n].tobytes(), issued)
+    return args, result, keep
+
+
+def anonymous_import(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, accounts, txs, g_epoch, proofs):
+    """import_anonymous_calls_block in one call (zk_import_anonymous_block): the issue rows, both verifications, the verdict
+    scatters and both state passes run on the device between one upload and one download, with the proofs checked on
+    ctx.  Same arguments, result and errors (conf_pvk may be None when the block has no issue), except that a key of
+    another shape raises SynthesisError(MalformedVerifyingKey) even when the block does not use it."""
+    args, result, _keep = _anon_section("anonymous_import", accounts, txs, g_epoch, proofs)
     for pvk in (anon_pvk, conf_pvk):
         if pvk is not None and pvk.ctx is not ctx:
             pvk.ctx.sync()
     try:
-        _ck(_lib.lib().zk_import_anonymous_block(ctx._h, anon_pvk._h, conf_pvk._h if conf_pvk is not None else None, n_acct, _p(buf(ky)),
-                                                 _p(buf(bal)), _p(buf(pend)), _p(buf(fl)), n, _p(buf(kind)), _p(mem),
-                                                 _p(buf(b"".join(t.points() for t in txs))), _p(buf(b"".join(t.rvk + t.nonce for t in txs))),
-                                                 _p(buf(fields)) if has_issue else None, _p(buf(ge)), _p(buf(proofs)), _p(v), _p(eb), _p(iss),
-                                                 _p(st), _p(nb), _p(npd), _p(nf)))
+        _ck(_lib.lib().zk_import_anonymous_block(ctx._h, anon_pvk._h, conf_pvk._h if conf_pvk is not None else None, *args))
     except ZkError as e:
         raise _import_error("anonymous_import", e) from None
-    issued = [iss[64 * k:64 * k + 64].tobytes() if kind[k] == ANON_ISSUE and st[k] == BLOCK_APPLIED else None for k in range(n)]
-    return ([int(x) for x in v[:n]], (nb[:64 * n_acct].tobytes(), npd[:64 * n_acct].tobytes(), nf[:n_acct].tobytes()),
-            eb[:64 * ANONIMITY_SIZE * n].tobytes(), issued)
+    return result()
 
 
 def anonymous_import_device(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_pvk: PreparedVerifyingKey, n_accounts: int, d_keys_ptr: int,
@@ -1359,6 +1393,104 @@ def anonymous_import_device(ctx: Context, anon_pvk: PreparedVerifyingKey, conf_p
                                                     v(d_g_epoch_ptr), v(d_proofs_ptr), v(d_verdicts_ptr), v(d_enc_balances_ptr),
                                                     v(d_issued_ptr), v(d_status_ptr), v(d_new_balances_ptr), v(d_new_pendings_ptr),
                                                     v(d_new_flags_ptr)))
+
+
+class BadSignature(ZkError):
+    """zk_import_block's ZK_ERR_BAD_SIGNATURE: extrinsic .index is the lowest whose signature fails, with the
+    redjubjub_verify verdict .verdict (0 / 2 / 3 / 4).  The block is invalid and nothing of it was applied."""
+
+    def __init__(self, code, msg, index: int, verdict: int):
+        super().__init__(code, msg)
+        self.index, self.verdict = index, verdict
+
+
+BlockImport = collections.namedtuple("BlockImport", "confidential assets anonymous launches")
+_BLOCK_SECTIONS = ("confidential", "assets", "anonymous")
+
+
+def _block_error(e: ZkError, first_bad: int):
+    """zk_import_block's errors as the sections' own calls raise them, with the section named"""
+    msg = str(e)
+    if e.code == _lib.ZK_ERR_BAD_SIGNATURE:
+        m = re.search(r"verdict (\d+)", msg)
+        return BadSignature(e.code, _lib.lib().zk_last_error().decode(), first_bad, int(m.group(1)))
+    for sec in _BLOCK_SECTIONS:
+        if ": %s: " % sec in msg:
+            name = "block_import: " + sec
+            return _asset_error(name, e) if sec == "assets" else _import_error(name, e)
+    return e
+
+
+def block_import(ctx: Context, conf_pvk: PreparedVerifyingKey, anon_pvk: PreparedVerifyingKey, signatures, confidential=None, assets=None,
+                 anonymous=None) -> BlockImport:
+    """A block's extrinsic signatures and the zk calls of all three pallets in one call (zk_import_block), with the
+    verifier launches the sections' data allow shared between them.
+    signatures: (vks, sigs, msgs, zs) as redjubjub_batch_verify takes them, one per extrinsic (zs None: drawn with
+    random_batch_scalars).  confidential: (accounts, txs, proofs) as confidential_import takes them; assets: (state, txs,
+    proofs, next_asset_id, new_slot_flags) as asset_calls_import; anonymous: (accounts, txs, g_epoch, proofs) as
+    anonymous_import.  None: the block has no such section.  conf_pvk / anon_pvk may be None where no section uses them.
+    Returns BlockImport: .confidential, .assets and .anonymous hold exactly what those functions return on their section
+    (None for an absent one), .launches the verifier launches made.  Raises BadSignature when an extrinsic's signature
+    fails (nothing is applied), and the sections' own errors, their ValueErrors named "block_import: <section>"."""
+    vks, sigs, msgs, zs = signatures
+    vk, sg = _cat(vks, 32), _cat(sigs, 64)
+    n_sig = len(msgs)
+    assert len(vk) == 32 * n_sig and len(sg) == 64 * n_sig
+    z = random_batch_scalars(n_sig) if zs is None else _cat(zs, 32)
+    assert len(z) == 32 * n_sig
+    buf = lambda b: np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+    sig_keep = [buf(vk), buf(sg), buf(b"".join(bytes(m) for m in msgs)), message_offsets(msgs), buf(z)]
+    sections = []
+    for sec, make, name in ((confidential, _conf_section, "confidential"), (assets, _asset_section, "assets"),
+                            (anonymous, _anon_section, "anonymous")):
+        if sec is None:
+            sections.append(None)
+            continue
+        sections.append(make("block_import: " + name, *sec))
+    # an absent section: zero sizes and NULL pointers (the asset one's n_slots_out still written)
+    n_out = C.c_size_t(0)
+    empty = ([0, None, None, None, 0] + [None] * 11,
+             [0] + [None] * 5 + [0, 0, 0] + [None] * 15 + [C.byref(n_out), None],
+             [0, None, None, None, None, 0] + [None] * 14)
+    args = []
+    for s, e in zip(sections, empty):
+        args += s[0] if s is not None else e
+    for pvk in (conf_pvk, anon_pvk):
+        if pvk is not None and pvk.ctx is not ctx:
+            pvk.ctx.sync()
+    first, launches = C.c_size_t(n_sig), C.c_uint(0)
+    try:
+        _ck(_lib.lib().zk_import_block(ctx._h, conf_pvk._h if conf_pvk is not None else None, anon_pvk._h if anon_pvk is not None else None,
+                                       n_sig, *[_p(a) for a in sig_keep], *args, C.byref(first), C.byref(launches)))
+    except ZkError as e:
+        raise _block_error(e, first.value) from None
+    out = [s[1]() if s is not None else None for s in sections]
+    return BlockImport(*out, launches.value)
+
+
+def block_import_device(ctx: Context, conf_pvk: PreparedVerifyingKey, anon_pvk: PreparedVerifyingKey, n_sig: int, d_vks_ptr: int,
+                        d_sigs_ptr: int, d_msgs_ptr: int, d_msg_off_ptr: int, d_zs_ptr: int, confidential, assets, anonymous):
+    """zk_import_block_device on device pointers.  The signatures as redjubjub_batch_verify_device takes them; confidential,
+    assets and anonymous: the arguments of confidential_import_device, asset_calls_import_device and
+    anonymous_import_device after their keys, as one tuple each (None: an absent section).  Blocks on the context's
+    stream as zk_import_block_device documents.  Returns (confidential rounds, (asset table rows, asset rounds),
+    launches), with the outputs complete; raises as block_import."""
+    v = lambda x: C.c_void_p(x) if x else None
+    c_rounds, a_rounds, n_out, first, launches = C.c_uint(0), C.c_uint(0), C.c_size_t(0), C.c_size_t(n_sig), C.c_uint(0)
+    c = list(confidential) if confidential is not None else [0] * 15
+    a = list(assets) if assets is not None else [0] * 24
+    n = list(anonymous) if anonymous is not None else [0] * 20
+    assert (len(c), len(a), len(n)) == (15, 24, 20)
+    c_args = [c[0]] + [v(x) for x in c[1:4]] + [c[4]] + [v(x) for x in c[5:]] + [C.byref(c_rounds)]
+    a_args = [a[0]] + [v(x) for x in a[1:6]] + [a[6], a[7] & 0xFF, a[8]] + [v(x) for x in a[9:]] + [C.byref(n_out), C.byref(a_rounds)]
+    n_args = [n[0]] + [v(x) for x in n[1:5]] + [n[5]] + [v(x) for x in n[6:]]
+    try:
+        _ck(_lib.lib().zk_import_block_device(ctx._h, conf_pvk._h if conf_pvk is not None else None,
+                                              anon_pvk._h if anon_pvk is not None else None, n_sig, v(d_vks_ptr), v(d_sigs_ptr), v(d_msgs_ptr),
+                                              v(d_msg_off_ptr), v(d_zs_ptr), *c_args, *a_args, *n_args, C.byref(first), C.byref(launches)))
+    except ZkError as e:
+        raise _block_error(e, first.value) from None
+    return c_rounds.value, (n_out.value, a_rounds.value), launches.value
 
 
 def pairing(ctx: Context, g1_uncompressed: bytes, g2_uncompressed: bytes) -> bytes:
