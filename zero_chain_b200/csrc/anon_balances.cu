@@ -244,58 +244,29 @@ static int check_args(const char *fn, zk_ctx *ctx, size_t n_accounts, const void
     return ZK_OK;
 }
 
-// the host forms: one staging buffer, inputs then outputs; kind NULL: no issue in the block
+// the host forms; kind NULL: no issue in the block
 static int host_block(zk_ctx *ctx, size_t n_accounts, const uint8_t *keys, const uint8_t *balances, const uint8_t *pendings,
                       const uint8_t *acct_flags, size_t n_tx, const uint8_t *kind, const uint32_t *members, const uint8_t *tx_points,
                       const uint8_t *tx_extra, const uint8_t *g_epoch, const uint8_t *applied, uint8_t *enc_balances, uint8_t *verify_points,
                       uint8_t *issued, uint8_t *tx_status, uint8_t *new_balances, uint8_t *new_pendings, uint8_t *new_flags) {
     if (!n_accounts && !n_tx) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    cudaStream_t st = ctx->stream;
-    const size_t vp_bytes = 32 * (size_t)AN_VERIFY_POINTS * n_tx, eb_bytes = 64 * (size_t)AN_RING * n_tx, nk = kind ? n_tx : 0;
-    // inputs, then outputs
-    Carve c;
-    for (int pass = 0; pass < 2; pass++) {
-        if (pass) c = Carve{ctx->bal_io.as<uint8_t>(), 0};
-        uint8_t *ky = c.take<uint8_t>(32 * n_accounts), *b = c.take<uint8_t>(64 * n_accounts), *p = c.take<uint8_t>(64 * n_accounts),
-                *f = c.take<uint8_t>(n_accounts);
-        uint32_t *m = c.take<uint32_t>(AN_RING * n_tx);
-        uint8_t *tp = c.take<uint8_t>(32 * AN_TX_POINTS * n_tx), *tx = c.take<uint8_t>(64 * n_tx), *ge = c.take<uint8_t>(32),
-                *ap = c.take<uint8_t>(n_tx), *eb = c.take<uint8_t>(eb_bytes), *vpt = c.take<uint8_t>(vp_bytes), *ts = c.take<uint8_t>(n_tx),
-                *nb = c.take<uint8_t>(64 * n_accounts), *npd = c.take<uint8_t>(64 * n_accounts), *nf = c.take<uint8_t>(n_accounts),
-                *kd = c.take<uint8_t>(nk), *is = c.take<uint8_t>(64 * nk);
-        if (!pass) { ZK_TRY(ctx->bal_io.reserve(c.off)); continue; }
-        if (n_accounts) {
-            ZK_CUDA(cudaMemcpyAsync(ky, keys, 32 * n_accounts, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(b, balances, 64 * n_accounts, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(p, pendings, 64 * n_accounts, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(f, acct_flags, n_accounts, cudaMemcpyHostToDevice, st));
-        }
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(m, members, 4 * AN_RING * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(tp, tx_points, 32 * AN_TX_POINTS * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(tx, tx_extra, 64 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ge, g_epoch, 32, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ap, applied, n_tx, cudaMemcpyHostToDevice, st));
-        }
-        if (nk) {
-            ZK_CUDA(cudaMemcpyAsync(kd, kind, nk, cudaMemcpyHostToDevice, st));
-            // the entries no applied issue writes keep the caller's bytes
-            ZK_CUDA(cudaMemcpyAsync(is, issued, 64 * nk, cudaMemcpyHostToDevice, st));
-        }
-        ZK_TRY(run_block(ctx, n_accounts, ky, b, p, f, n_tx, nk ? kd : nullptr, m, tp, tx, ge, ap, eb, vpt, is, ts, nb, npd, nf, ctx->bal));
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(enc_balances, eb, eb_bytes, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(verify_points, vpt, vp_bytes, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(tx_status, ts, n_tx, cudaMemcpyDeviceToHost, st));
-        }
-        if (nk) ZK_CUDA(cudaMemcpyAsync(issued, is, 64 * nk, cudaMemcpyDeviceToHost, st));
-        if (n_accounts) {
-            ZK_CUDA(cudaMemcpyAsync(new_balances, nb, 64 * n_accounts, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_pendings, npd, 64 * n_accounts, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_flags, nf, n_accounts, cudaMemcpyDeviceToHost, st));
-        }
-    }
+    const size_t nk = kind ? n_tx : 0;
+    const uint8_t *ky, *b, *p, *f, *kd, *tp, *tx, *ge, *ap;
+    const uint32_t *m;
+    uint8_t *eb, *vpt, *is, *ts, *nb, *npd, *nf;
+    Stage io;
+    io.in(keys, ky, 32 * n_accounts); io.in(balances, b, 64 * n_accounts); io.in(pendings, p, 64 * n_accounts);
+    io.in(acct_flags, f, n_accounts);
+    io.in(kind, kd, nk); io.in(members, m, AN_RING * n_tx); io.in(tx_points, tp, 32 * AN_TX_POINTS * n_tx); io.in(tx_extra, tx, 64 * n_tx);
+    io.in(g_epoch, ge, n_tx ? 32 : 0); io.in(applied, ap, n_tx);
+    io.out(enc_balances, eb, 64 * (size_t)AN_RING * n_tx); io.out(verify_points, vpt, 32 * (size_t)AN_VERIFY_POINTS * n_tx);
+    io.inout(issued, is, 64 * nk);                // the entries no applied issue writes keep the caller's bytes
+    io.out(tx_status, ts, n_tx);
+    io.out(new_balances, nb, 64 * n_accounts); io.out(new_pendings, npd, 64 * n_accounts); io.out(new_flags, nf, n_accounts);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(run_block(ctx, n_accounts, ky, b, p, f, n_tx, kd, m, tp, tx, ge, ap, eb, vpt, is, ts, nb, npd, nf, ctx->bal));
+    ZK_TRY(io.down(ctx));
     return zk_check_err_flag(ctx);     // synchronises the stream; ZK_ERR_DECODE names a touched account that failed to read
 }
 

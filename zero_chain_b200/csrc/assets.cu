@@ -226,45 +226,19 @@ extern "C" int zk_assets_block(zk_ctx *ctx, size_t n_slots, const uint8_t *balan
                       balance_sender, balance_after, event_ct, event_flags, tx_status, new_balances, new_pendings, new_flags));
     if (!n_slots && !n_tx) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    cudaStream_t st = ctx->stream;
-    // inputs, then outputs; balance_after, event_ct and event_flags go up too, since only some of their entries are written
-    Carve c;
-    for (int pass = 0; pass < 2; pass++) {
-        if (pass) c = Carve{ctx->bal_io.as<uint8_t>(), 0};
-        uint8_t *b = c.take<uint8_t>(64 * n_slots), *p = c.take<uint8_t>(64 * n_slots), *f = c.take<uint8_t>(n_slots);
-        uint32_t *sa = c.take<uint32_t>(n_tx), *sb = c.take<uint32_t>(n_tx);
-        uint8_t *kd = c.take<uint8_t>(n_tx), *tp = c.take<uint8_t>(128 * n_tx), *ap = c.take<uint8_t>(n_tx), *bs = c.take<uint8_t>(64 * n_tx),
-                *ba = c.take<uint8_t>(64 * n_tx), *ev = c.take<uint8_t>(128 * n_tx), *ef = c.take<uint8_t>(n_tx), *ts = c.take<uint8_t>(n_tx),
-                *nb = c.take<uint8_t>(64 * n_slots), *npd = c.take<uint8_t>(64 * n_slots), *nf = c.take<uint8_t>(n_slots);
-        if (!pass) { ZK_TRY(ctx->bal_io.reserve(c.off)); continue; }
-        if (n_slots) {
-            ZK_CUDA(cudaMemcpyAsync(b, balances, 64 * n_slots, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(p, pendings, 64 * n_slots, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(f, slot_flags, n_slots, cudaMemcpyHostToDevice, st));
-        }
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(kd, kind, n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(sa, slot_a, 4 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(sb, slot_b, 4 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(tp, tx_points, 128 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ap, applied, n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ba, balance_after, 64 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ev, event_ct, 128 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ef, event_flags, n_tx, cudaMemcpyHostToDevice, st));
-        }
-        ZK_TRY(run_block(ctx, n_slots, b, p, f, n_tx, kd, sa, sb, tp, ap, bs, ba, ev, ef, ts, nb, npd, nf, ctx->bal));
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(balance_sender, bs, 64 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(balance_after, ba, 64 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(event_ct, ev, 128 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(event_flags, ef, n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(tx_status, ts, n_tx, cudaMemcpyDeviceToHost, st));
-        }
-        if (n_slots) {
-            ZK_CUDA(cudaMemcpyAsync(new_balances, nb, 64 * n_slots, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_pendings, npd, 64 * n_slots, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_flags, nf, n_slots, cudaMemcpyDeviceToHost, st));
-        }
-    }
+    const uint8_t *b, *p, *f, *kd, *tp, *ap;
+    const uint32_t *sa, *sb;
+    uint8_t *bs, *ba, *ev, *ef, *ts, *nb, *npd, *nf;
+    Stage io;
+    io.in(balances, b, 64 * n_slots); io.in(pendings, p, 64 * n_slots); io.in(slot_flags, f, n_slots);
+    io.in(kind, kd, n_tx); io.in(slot_a, sa, n_tx); io.in(slot_b, sb, n_tx); io.in(tx_points, tp, 128 * n_tx); io.in(applied, ap, n_tx);
+    io.out(balance_sender, bs, 64 * n_tx);
+    // only some of these entries are written
+    io.inout(balance_after, ba, 64 * n_tx); io.inout(event_ct, ev, 128 * n_tx); io.inout(event_flags, ef, n_tx);
+    io.out(tx_status, ts, n_tx);
+    io.out(new_balances, nb, 64 * n_slots); io.out(new_pendings, npd, 64 * n_slots); io.out(new_flags, nf, n_slots);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(run_block(ctx, n_slots, b, p, f, n_tx, kd, sa, sb, tp, ap, bs, ba, ev, ef, ts, nb, npd, nf, ctx->bal));
+    ZK_TRY(io.down(ctx));
     return zk_check_err_flag(ctx);     // synchronises the stream; ZK_ERR_DECODE names a touched slot that failed to read
 }

@@ -308,40 +308,18 @@ extern "C" int zk_balances_confidential_block(zk_ctx *ctx, size_t n_accounts, co
                       tx_points, applied, balance_sender, balance_after, tx_status, new_balances, new_pendings, new_flags));
     if (!n_accounts && !n_tx) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    cudaStream_t st = ctx->stream;
-    // inputs, then outputs; balance_after goes up too, since only the applied transactions' entries are written
-    Carve c;
-    for (int pass = 0; pass < 2; pass++) {
-        if (pass) c = Carve{ctx->bal_io.as<uint8_t>(), 0};
-        uint8_t *b = c.take<uint8_t>(64 * n_accounts), *p = c.take<uint8_t>(64 * n_accounts), *f = c.take<uint8_t>(n_accounts);
-        uint32_t *s = c.take<uint32_t>(n_tx), *r = c.take<uint32_t>(n_tx);
-        uint8_t *tp = c.take<uint8_t>(128 * n_tx), *ap = c.take<uint8_t>(n_tx), *bs = c.take<uint8_t>(64 * n_tx), *ba = c.take<uint8_t>(64 * n_tx),
-                *ts = c.take<uint8_t>(n_tx), *nb = c.take<uint8_t>(64 * n_accounts), *npd = c.take<uint8_t>(64 * n_accounts),
-                *nf = c.take<uint8_t>(n_accounts);
-        if (!pass) { ZK_TRY(ctx->bal_io.reserve(c.off)); continue; }
-        if (n_accounts) {
-            ZK_CUDA(cudaMemcpyAsync(b, balances, 64 * n_accounts, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(p, pendings, 64 * n_accounts, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(f, acct_flags, n_accounts, cudaMemcpyHostToDevice, st));
-        }
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(s, sender, 4 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(r, recipient, 4 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(tp, tx_points, 128 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ap, applied, n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(ba, balance_after, 64 * n_tx, cudaMemcpyHostToDevice, st));
-        }
-        ZK_TRY(run_block(ctx, n_accounts, b, p, f, n_tx, s, r, tp, ap, bs, ba, ts, nb, npd, nf, ctx->bal));
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(balance_sender, bs, 64 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(balance_after, ba, 64 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(tx_status, ts, n_tx, cudaMemcpyDeviceToHost, st));
-        }
-        if (n_accounts) {
-            ZK_CUDA(cudaMemcpyAsync(new_balances, nb, 64 * n_accounts, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_pendings, npd, 64 * n_accounts, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_flags, nf, n_accounts, cudaMemcpyDeviceToHost, st));
-        }
-    }
+    const uint8_t *b, *p, *f, *tp, *ap;
+    const uint32_t *s, *r;
+    uint8_t *bs, *ba, *ts, *nb, *npd, *nf;
+    Stage io;
+    io.in(balances, b, 64 * n_accounts); io.in(pendings, p, 64 * n_accounts); io.in(acct_flags, f, n_accounts);
+    io.in(sender, s, n_tx); io.in(recipient, r, n_tx); io.in(tx_points, tp, 128 * n_tx); io.in(applied, ap, n_tx);
+    io.out(balance_sender, bs, 64 * n_tx);
+    io.inout(balance_after, ba, 64 * n_tx);       // only the applied transactions' entries are written
+    io.out(tx_status, ts, n_tx);
+    io.out(new_balances, nb, 64 * n_accounts); io.out(new_pendings, npd, 64 * n_accounts); io.out(new_flags, nf, n_accounts);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(run_block(ctx, n_accounts, b, p, f, n_tx, s, r, tp, ap, bs, ba, ts, nb, npd, nf, ctx->bal));
+    ZK_TRY(io.down(ctx));
     return zk_check_err_flag(ctx);     // synchronises the stream; ZK_ERR_DECODE names a touched account that failed to read
 }

@@ -83,16 +83,15 @@ extern "C" int zk_elgamal_decrypt_batch(zk_ctx *ctx, size_t n, const uint8_t *dk
     }
     if (!n) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    const size_t pend_bytes = pending ? 64 * n : 0;
-    ZK_TRY(ctx->v_io.reserve(4 * n + 32 * n + 64 * n + pend_bytes + n));
-    uint8_t *d_values = ctx->v_io.as<uint8_t>(), *d_dks = d_values + 4 * n, *d_cts = d_dks + 32 * n, *d_pend = d_cts + 64 * n,
-            *d_status = d_pend + pend_bytes;
-    ZK_CUDA(cudaMemcpyAsync(d_dks, dks, 32 * n, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d_cts, cts, 64 * n, cudaMemcpyHostToDevice, ctx->stream));
-    if (pending) ZK_CUDA(cudaMemcpyAsync(d_pend, pending, pend_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_TRY(launch_decrypt(ctx, n, d_dks, d_cts, pending ? d_pend : nullptr, reinterpret_cast<uint32_t *>(d_values), d_status));
-    ZK_CUDA(cudaMemcpyAsync(values, d_values, 4 * n, cudaMemcpyDeviceToHost, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(status, d_status, n, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint8_t *d_dks, *d_cts, *d_pend;
+    uint32_t *d_values;
+    uint8_t *d_status;
+    Stage io;
+    io.in(dks, d_dks, 32 * n); io.in(cts, d_cts, 64 * n); io.in(pending, d_pend, 64 * n);
+    io.out(values, d_values, n); io.out(status, d_status, n);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(launch_decrypt(ctx, n, d_dks, d_cts, d_pend, d_values, d_status));
+    ZK_TRY(io.down(ctx));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     return ZK_OK;
 }

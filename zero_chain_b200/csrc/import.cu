@@ -5,7 +5,7 @@
 // between the first upload and the last download; the host reads a block of counters only where the next launch's size
 // depends on it.
 //
-// The round buffers live in the context (ctx->imp, ctx->imp_as); the host forms stage their arrays in ctx->imp_io.
+// The round buffers live in the context (ctx->imp, ctx->imp_as); the host forms stage their arrays in ctx->io (Stage).
 #include "internal.h"
 #include "anon_balances.cuh"
 #include "assets.cuh"
@@ -399,102 +399,43 @@ static int anon_args(const AnonIn &a) {
 }
 
 // ---- the host forms' staging --------------------------------------------------------------------------------------------
-// stage(c, h, d): d = h with every array replaced by its place in ctx->imp_io (c sizes with a null base); up(): the
-// inputs to the device; down(): the outputs back.
-template <class T> static T *place(Carve &c, const T *h, size_t count) { return h ? c.take<T>(count) : nullptr; }
-template <class T> static int up(zk_ctx *ctx, const T *d, const T *h, size_t count) {
-    if (count && h) ZK_CUDA(cudaMemcpyAsync((void *)d, h, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-    return ZK_OK;
-}
-template <class T> static int down(zk_ctx *ctx, T *h, const T *d, size_t count) {
-    if (count && h) ZK_CUDA(cudaMemcpyAsync(h, d, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
-    return ZK_OK;
-}
-
-static void stage(Carve &c, const ConfIn &h, ConfIn &d) {
+// stage(io, h, d): d = h with every array registered in io, which puts its device copy in its place
+static void stage(Stage &io, const ConfIn &h, ConfIn &d) {
     const size_t na = h.n_accounts, n = h.n_tx;
     d = h;
-    d.balances = place(c, h.balances, 64 * na); d.pendings = place(c, h.pendings, 64 * na); d.acct_flags = place(c, h.acct_flags, na);
-    d.sender = place(c, h.sender, n); d.recipient = place(c, h.recipient, n);
-    d.rows = place(c, h.rows, IMP_ROW * n); d.proofs = place(c, h.proofs, 192 * n);
-    d.verdicts = place(c, h.verdicts, n); d.balance_after = place(c, h.balance_after, 64 * n); d.tx_status = place(c, h.tx_status, n);
-    d.new_balances = place(c, h.new_balances, 64 * na); d.new_pendings = place(c, h.new_pendings, 64 * na);
-    d.new_flags = place(c, h.new_flags, na);
+    io.in(h.balances, d.balances, 64 * na); io.in(h.pendings, d.pendings, 64 * na); io.in(h.acct_flags, d.acct_flags, na);
+    io.in(h.sender, d.sender, n); io.in(h.recipient, d.recipient, n);
+    io.in(h.rows, d.rows, IMP_ROW * n); io.in(h.proofs, d.proofs, 192 * n);
+    io.out(h.verdicts, d.verdicts, n); io.out(h.balance_after, d.balance_after, 64 * n); io.out(h.tx_status, d.tx_status, n);
+    io.out(h.new_balances, d.new_balances, 64 * na); io.out(h.new_pendings, d.new_pendings, 64 * na);
+    io.out(h.new_flags, d.new_flags, na);
 }
-static int up(zk_ctx *ctx, const ConfIn &d, const ConfIn &h) {
-    const size_t na = h.n_accounts, n = h.n_tx;
-    ZK_TRY(up(ctx, d.balances, h.balances, 64 * na)); ZK_TRY(up(ctx, d.pendings, h.pendings, 64 * na));
-    ZK_TRY(up(ctx, d.acct_flags, h.acct_flags, na)); ZK_TRY(up(ctx, d.sender, h.sender, n)); ZK_TRY(up(ctx, d.recipient, h.recipient, n));
-    ZK_TRY(up(ctx, d.rows, h.rows, IMP_ROW * n));
-    return up(ctx, d.proofs, h.proofs, 192 * n);
-}
-static int down(zk_ctx *ctx, const ConfIn &h, const ConfIn &d) {
-    const size_t na = h.n_accounts, n = h.n_tx;
-    ZK_TRY(down(ctx, h.verdicts, d.verdicts, n)); ZK_TRY(down(ctx, h.balance_after, d.balance_after, 64 * n));
-    ZK_TRY(down(ctx, h.tx_status, d.tx_status, n)); ZK_TRY(down(ctx, h.new_balances, d.new_balances, 64 * na));
-    ZK_TRY(down(ctx, h.new_pendings, d.new_pendings, 64 * na));
-    return down(ctx, h.new_flags, d.new_flags, na);
-}
-
-static void stage(Carve &c, const AssetIn &h, AssetIn &d) {
+// the grown table has room for a new row at every reference; *n_out of its rows come down
+static void stage(Stage &io, const AssetIn &h, AssetIn &d, size_t *n_out) {
     const size_t ns = h.n_slots, n = h.n_tx, nr = h.n_slots + 2 * h.n_tx;
     d = h;
-    d.slot_ids = place(c, h.slot_ids, ns); d.slot_keys = place(c, h.slot_keys, 32 * ns); d.balances = place(c, h.balances, 64 * ns);
-    d.pendings = place(c, h.pendings, 64 * ns); d.slot_flags = place(c, h.slot_flags, ns);
-    d.kind = place(c, h.kind, n); d.asset_id = place(c, h.asset_id, n); d.rows = place(c, h.rows, IMP_ROW * n);
-    d.proofs = place(c, h.proofs, 192 * n); d.verdicts = place(c, h.verdicts, n); d.asset_ids = place(c, h.asset_ids, n);
-    d.balance_after = place(c, h.balance_after, 64 * n); d.event_ct = place(c, h.event_ct, 128 * n);
-    d.event_flags = place(c, h.event_flags, n); d.tx_status = place(c, h.tx_status, n);
-    d.new_slot_ids = place(c, h.new_slot_ids, nr); d.new_slot_keys = place(c, h.new_slot_keys, 32 * nr);
-    d.new_balances = place(c, h.new_balances, 64 * nr); d.new_pendings = place(c, h.new_pendings, 64 * nr);
-    d.new_flags = place(c, h.new_flags, nr);
+    d.n_slots_out = n_out;
+    io.in(h.slot_ids, d.slot_ids, ns); io.in(h.slot_keys, d.slot_keys, 32 * ns); io.in(h.balances, d.balances, 64 * ns);
+    io.in(h.pendings, d.pendings, 64 * ns); io.in(h.slot_flags, d.slot_flags, ns);
+    io.in(h.kind, d.kind, n); io.in(h.asset_id, d.asset_id, n); io.in(h.rows, d.rows, IMP_ROW * n); io.in(h.proofs, d.proofs, 192 * n);
+    io.out(h.verdicts, d.verdicts, n); io.out(h.asset_ids, d.asset_ids, n);
+    io.out(h.balance_after, d.balance_after, 64 * n); io.out(h.event_ct, d.event_ct, 128 * n);
+    io.out(h.event_flags, d.event_flags, n); io.out(h.tx_status, d.tx_status, n);
+    io.out(h.new_slot_ids, d.new_slot_ids, nr, n_out); io.out(h.new_slot_keys, d.new_slot_keys, 32 * nr, n_out, 32);
+    io.out(h.new_balances, d.new_balances, 64 * nr, n_out, 64); io.out(h.new_pendings, d.new_pendings, 64 * nr, n_out, 64);
+    io.out(h.new_flags, d.new_flags, nr, n_out);
 }
-static int up(zk_ctx *ctx, const AssetIn &d, const AssetIn &h) {
-    const size_t ns = h.n_slots, n = h.n_tx;
-    ZK_TRY(up(ctx, d.slot_ids, h.slot_ids, ns)); ZK_TRY(up(ctx, d.slot_keys, h.slot_keys, 32 * ns));
-    ZK_TRY(up(ctx, d.balances, h.balances, 64 * ns)); ZK_TRY(up(ctx, d.pendings, h.pendings, 64 * ns));
-    ZK_TRY(up(ctx, d.slot_flags, h.slot_flags, ns)); ZK_TRY(up(ctx, d.kind, h.kind, n)); ZK_TRY(up(ctx, d.asset_id, h.asset_id, n));
-    ZK_TRY(up(ctx, d.rows, h.rows, IMP_ROW * n));
-    return up(ctx, d.proofs, h.proofs, 192 * n);
-}
-// n_out: the grown table's rows
-static int down(zk_ctx *ctx, const AssetIn &h, const AssetIn &d, size_t n_out) {
-    const size_t n = h.n_tx;
-    ZK_TRY(down(ctx, h.verdicts, d.verdicts, n)); ZK_TRY(down(ctx, h.asset_ids, d.asset_ids, n));
-    ZK_TRY(down(ctx, h.balance_after, d.balance_after, 64 * n)); ZK_TRY(down(ctx, h.event_ct, d.event_ct, 128 * n));
-    ZK_TRY(down(ctx, h.event_flags, d.event_flags, n)); ZK_TRY(down(ctx, h.tx_status, d.tx_status, n));
-    ZK_TRY(down(ctx, h.new_slot_ids, d.new_slot_ids, n_out)); ZK_TRY(down(ctx, h.new_slot_keys, d.new_slot_keys, 32 * n_out));
-    ZK_TRY(down(ctx, h.new_balances, d.new_balances, 64 * n_out)); ZK_TRY(down(ctx, h.new_pendings, d.new_pendings, 64 * n_out));
-    return down(ctx, h.new_flags, d.new_flags, n_out);
-}
-
-static void stage(Carve &c, const AnonIn &h, AnonIn &d) {
+static void stage(Stage &io, const AnonIn &h, AnonIn &d) {
     const size_t na = h.n_accounts, n = h.n_tx;
     d = h;
-    d.keys = place(c, h.keys, 32 * na); d.balances = place(c, h.balances, 64 * na); d.pendings = place(c, h.pendings, 64 * na);
-    d.acct_flags = place(c, h.acct_flags, na); d.kind = place(c, h.kind, n); d.members = place(c, h.members, IMP_AN_RING * n);
-    d.tx_points = place(c, h.tx_points, 32 * (size_t)IMP_AN_TX_POINTS * n); d.tx_extra = place(c, h.tx_extra, 64 * n);
-    d.issue_fields = place(c, h.issue_fields, 96 * n); d.g_epoch = place(c, h.g_epoch, 32); d.proofs = place(c, h.proofs, 192 * n);
-    d.verdicts = place(c, h.verdicts, n); d.enc_balances = place(c, h.enc_balances, 64 * (size_t)IMP_AN_RING * n);
-    d.issued = place(c, h.issued, 64 * n); d.tx_status = place(c, h.tx_status, n);
-    d.new_balances = place(c, h.new_balances, 64 * na); d.new_pendings = place(c, h.new_pendings, 64 * na);
-    d.new_flags = place(c, h.new_flags, na);
-}
-static int up(zk_ctx *ctx, const AnonIn &d, const AnonIn &h) {
-    const size_t na = h.n_accounts, n = h.n_tx;
-    ZK_TRY(up(ctx, d.keys, h.keys, 32 * na)); ZK_TRY(up(ctx, d.balances, h.balances, 64 * na));
-    ZK_TRY(up(ctx, d.pendings, h.pendings, 64 * na)); ZK_TRY(up(ctx, d.acct_flags, h.acct_flags, na));
-    ZK_TRY(up(ctx, d.kind, h.kind, n)); ZK_TRY(up(ctx, d.members, h.members, IMP_AN_RING * n));
-    ZK_TRY(up(ctx, d.tx_points, h.tx_points, 32 * (size_t)IMP_AN_TX_POINTS * n)); ZK_TRY(up(ctx, d.tx_extra, h.tx_extra, 64 * n));
-    ZK_TRY(up(ctx, d.issue_fields, h.issue_fields, 96 * n)); ZK_TRY(up(ctx, d.g_epoch, h.g_epoch, n ? 32 : 0));
-    return up(ctx, d.proofs, h.proofs, 192 * n);
-}
-static int down(zk_ctx *ctx, const AnonIn &h, const AnonIn &d) {
-    const size_t na = h.n_accounts, n = h.n_tx;
-    ZK_TRY(down(ctx, h.verdicts, d.verdicts, n)); ZK_TRY(down(ctx, h.enc_balances, d.enc_balances, 64 * (size_t)IMP_AN_RING * n));
-    ZK_TRY(down(ctx, h.issued, d.issued, 64 * n)); ZK_TRY(down(ctx, h.tx_status, d.tx_status, n));
-    ZK_TRY(down(ctx, h.new_balances, d.new_balances, 64 * na)); ZK_TRY(down(ctx, h.new_pendings, d.new_pendings, 64 * na));
-    return down(ctx, h.new_flags, d.new_flags, na);
+    io.in(h.keys, d.keys, 32 * na); io.in(h.balances, d.balances, 64 * na); io.in(h.pendings, d.pendings, 64 * na);
+    io.in(h.acct_flags, d.acct_flags, na); io.in(h.kind, d.kind, n); io.in(h.members, d.members, IMP_AN_RING * n);
+    io.in(h.tx_points, d.tx_points, 32 * (size_t)IMP_AN_TX_POINTS * n); io.in(h.tx_extra, d.tx_extra, 64 * n);
+    io.in(h.issue_fields, d.issue_fields, 96 * n); io.in(h.g_epoch, d.g_epoch, n ? 32 : 0); io.in(h.proofs, d.proofs, 192 * n);
+    io.out(h.verdicts, d.verdicts, n); io.out(h.enc_balances, d.enc_balances, 64 * (size_t)IMP_AN_RING * n);
+    io.out(h.issued, d.issued, 64 * n); io.out(h.tx_status, d.tx_status, n);
+    io.out(h.new_balances, d.new_balances, 64 * na); io.out(h.new_pendings, d.new_pendings, 64 * na);
+    io.out(h.new_flags, d.new_flags, na);
 }
 
 // ---- one block --------------------------------------------------------------------------------------------------------
@@ -784,48 +725,31 @@ static int block_run(zk_ctx *ctx, const zk_pvk *conf_pvk, const zk_pvk *anon_pvk
     return ZK_OK;
 }
 
-// The host forms: every section staged in ctx->imp_io, the engine, the outputs back.  The signatures' offsets go up
-// counted from the first message.
+// The host forms: every section staged in ctx->io, the engine, the outputs back.  The messages go up from the first
+// one, their offsets counted from it.
 static int host_run(zk_ctx *ctx, const zk_pvk *conf_pvk, const zk_pvk *anon_pvk, const SigIn *sg, const ConfIn *ci, const AssetIn *ai,
                     const AnonIn *ni, size_t *first_bad_sig, unsigned *launches) {
-    cudaStream_t st = ctx->stream;
     SigIn ds{};
     ConfIn dc{};
     AssetIn da{};
     AnonIn dn{};
-    const size_t n_sig = sg ? sg->n : 0, msg_bytes = n_sig ? sg->msg_off[n_sig] - sg->msg_off[0] : 0;
-    std::vector<uint64_t> off(n_sig + 1);
-    for (size_t i = 0; i < off.size() && n_sig; i++) off[i] = sg->msg_off[i] - sg->msg_off[0];
-    auto stage_all = [&](Carve &c) {
-        if (n_sig) {
-            ds.n = n_sig;
-            ds.vks = c.take<uint8_t>(32 * n_sig); ds.sigs = c.take<uint8_t>(64 * n_sig); ds.zs = c.take<uint8_t>(32 * n_sig);
-            ds.msgs = c.take<uint8_t>(msg_bytes ? msg_bytes : 1); ds.msg_off = c.take<uint64_t>(n_sig + 1);
-        }
-        if (ci) stage(c, *ci, dc);
-        if (ai) stage(c, *ai, da);
-        if (ni) stage(c, *ni, dn);
-        return c.off;
-    };
-    Carve sizing;
-    ZK_TRY(ctx->imp_io.reserve(stage_all(sizing)));
-    Carve c{ctx->imp_io.as<uint8_t>(), 0};
-    stage_all(c);
-    if (n_sig) {
-        ZK_TRY(up(ctx, ds.vks, sg->vks, 32 * n_sig)); ZK_TRY(up(ctx, ds.sigs, sg->sigs, 64 * n_sig)); ZK_TRY(up(ctx, ds.zs, sg->zs, 32 * n_sig));
-        ZK_TRY(up(ctx, ds.msgs, sg->msgs + sg->msg_off[0], msg_bytes)); ZK_TRY(up(ctx, ds.msg_off, off.data(), n_sig + 1));
-    }
-    if (ci) ZK_TRY(up(ctx, dc, *ci));
-    if (ai) ZK_TRY(up(ctx, da, *ai));
-    if (ni) ZK_TRY(up(ctx, dn, *ni));
     size_t n_out = 0;
-    da.n_slots_out = &n_out;
-    ZK_TRY(block_run(ctx, conf_pvk, anon_pvk, n_sig ? &ds : nullptr, ci ? &dc : nullptr, ai ? &da : nullptr, ni ? &dn : nullptr, first_bad_sig,
+    std::vector<uint64_t> off;
+    Stage io;
+    if (sg) {
+        ds.n = sg->n;
+        for (size_t i = 0; i <= sg->n; i++) off.push_back(sg->msg_off[i] - sg->msg_off[0]);
+        io.in(sg->vks, ds.vks, 32 * sg->n); io.in(sg->sigs, ds.sigs, 64 * sg->n); io.in(sg->zs, ds.zs, 32 * sg->n);
+        io.in(sg->msgs + sg->msg_off[0], ds.msgs, off[sg->n]); io.in(off.data(), ds.msg_off, sg->n + 1);
+    }
+    if (ci) stage(io, *ci, dc);
+    if (ai) stage(io, *ai, da, &n_out);
+    if (ni) stage(io, *ni, dn);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(block_run(ctx, conf_pvk, anon_pvk, sg ? &ds : nullptr, ci ? &dc : nullptr, ai ? &da : nullptr, ni ? &dn : nullptr, first_bad_sig,
                      launches));
-    if (ci) ZK_TRY(down(ctx, *ci, dc));
-    if (ai) ZK_TRY(down(ctx, *ai, da, n_out));
-    if (ni) ZK_TRY(down(ctx, *ni, dn));
-    ZK_CUDA(cudaStreamSynchronize(st));
+    ZK_TRY(io.down(ctx));
+    ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     if (ai) *ai->n_slots_out = n_out;
     return ZK_OK;
 }
@@ -976,47 +900,20 @@ extern "C" int zk_import_assets_block(zk_ctx *ctx, const zk_pvk *pvk, size_t n_s
     if (rounds) *rounds = 0;
     if (!n_slots && !n_tx) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    cudaStream_t st = ctx->stream;
-    const size_t ns = n_slots;
-    Carve c;
-    for (int pass = 0; pass < 2; pass++) {     // inputs, then outputs
-        if (pass) c = Carve{ctx->imp_io.as<uint8_t>(), 0};
-        uint8_t *b = c.take<uint8_t>(64 * ns), *p = c.take<uint8_t>(64 * ns), *f = c.take<uint8_t>(ns);
-        uint32_t *sa = c.take<uint32_t>(n_tx), *sb = c.take<uint32_t>(n_tx);
-        uint8_t *kd = c.take<uint8_t>(n_tx), *tp = c.take<uint8_t>(128 * n_tx), *rw = c.take<uint8_t>(IMP_ROW * n_tx),
-                *pf = c.take<uint8_t>(192 * n_tx), *fx = c.take<uint8_t>(n_tx), *v = c.take<uint8_t>(n_tx), *ba = c.take<uint8_t>(64 * n_tx),
-                *ev = c.take<uint8_t>(128 * n_tx), *ef = c.take<uint8_t>(n_tx), *ts = c.take<uint8_t>(n_tx), *nb = c.take<uint8_t>(64 * ns),
-                *npd = c.take<uint8_t>(64 * ns), *nf = c.take<uint8_t>(ns);
-        if (!pass) { ZK_TRY(ctx->imp_io.reserve(c.off)); continue; }
-        if (ns) {
-            ZK_CUDA(cudaMemcpyAsync(b, balances, 64 * ns, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(p, pendings, 64 * ns, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(f, slot_flags, ns, cudaMemcpyHostToDevice, st));
-        }
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(sa, slot_a, 4 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(sb, slot_b, 4 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(kd, kind, n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(tp, tx_points, 128 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(rw, rows, IMP_ROW * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(pf, proofs, 192 * n_tx, cudaMemcpyHostToDevice, st));
-            ZK_CUDA(cudaMemcpyAsync(fx, fixed_verdicts, n_tx, cudaMemcpyHostToDevice, st));
-        }
-        ZK_TRY(assets_run(ctx, fn, pvk, ns, b, p, f, n_tx, kd, sa, sb, tp, rw, pf, fx, v, ba, ev, ef, ts, nb, npd, nf, rounds));
-        if (n_tx) {
-            ZK_CUDA(cudaMemcpyAsync(verdicts, v, n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(balance_after, ba, 64 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(event_ct, ev, 128 * n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(event_flags, ef, n_tx, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(tx_status, ts, n_tx, cudaMemcpyDeviceToHost, st));
-        }
-        if (ns) {
-            ZK_CUDA(cudaMemcpyAsync(new_balances, nb, 64 * ns, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_pendings, npd, 64 * ns, cudaMemcpyDeviceToHost, st));
-            ZK_CUDA(cudaMemcpyAsync(new_flags, nf, ns, cudaMemcpyDeviceToHost, st));
-        }
-    }
-    ZK_CUDA(cudaStreamSynchronize(st));
+    const uint8_t *b, *p, *f, *kd, *tp, *rw, *pf, *fx;
+    const uint32_t *sa, *sb;
+    uint8_t *v, *ba, *ev, *ef, *ts, *nb, *npd, *nf;
+    Stage io;
+    io.in(balances, b, 64 * n_slots); io.in(pendings, p, 64 * n_slots); io.in(slot_flags, f, n_slots);
+    io.in(slot_a, sa, n_tx); io.in(slot_b, sb, n_tx); io.in(kind, kd, n_tx); io.in(tx_points, tp, 128 * n_tx);
+    io.in(rows, rw, IMP_ROW * n_tx); io.in(proofs, pf, 192 * n_tx); io.in(fixed_verdicts, fx, n_tx);
+    io.out(verdicts, v, n_tx); io.out(balance_after, ba, 64 * n_tx); io.out(event_ct, ev, 128 * n_tx); io.out(event_flags, ef, n_tx);
+    io.out(tx_status, ts, n_tx);
+    io.out(new_balances, nb, 64 * n_slots); io.out(new_pendings, npd, 64 * n_slots); io.out(new_flags, nf, n_slots);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(assets_run(ctx, fn, pvk, n_slots, b, p, f, n_tx, kd, sa, sb, tp, rw, pf, fx, v, ba, ev, ef, ts, nb, npd, nf, rounds));
+    ZK_TRY(io.down(ctx));
+    ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     return ZK_OK;
 }
 

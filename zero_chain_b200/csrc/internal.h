@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <string>
+#include <type_traits>
 #include <vector>
 #include "../../include/zkb200.h"
 
@@ -80,15 +81,16 @@ struct zk_ctx {
     // groth16 workspace
     DevBuf g_a, g_b, g_c, g_h, g_scal, g_misc;
     // verifier workspace (pairing.cu)
-    DevBuf v_pts, v_stat, v_coef, v_f, v_part, v_io;
+    DevBuf v_pts, v_stat, v_coef, v_f, v_part;
     DevBuf v_jj;                   // zk_groth16_verify_points_batch: decoded public inputs and per-point status (jubjub.cu)
     // zk_elgamal_decrypt_batch (elgamal.cu): the encodings of i P_G for i < 10^6 and their index, built by the first call
     DevBuf eg_table, eg_index;
     bool eg_ready = false;
-    DevBuf bal, bal_io;            // zk_balances_confidential_block (balances.cu), zk_balances_anonymous_block
-                                   // (anon_balances.cu) and zk_assets_block (assets.cu): workspace, and the host forms' staging
-    DevBuf imp, imp_io;            // zk_import_confidential_block / zk_import_assets_block (import.cu): round buffers, and
-                                   // the host forms' staging
+    DevBuf bal;                    // zk_balances_confidential_block (balances.cu), zk_balances_anonymous_block
+                                   // (anon_balances.cu) and zk_assets_block (assets.cu): workspace
+    DevBuf imp;                    // zk_import_confidential_block / zk_import_assets_block (import.cu): round buffers
+    DevBuf io;                     // the host forms' arrays (Stage); no device form reads it, and every host form
+                                   // synchronises before it returns, so one buffer serves them all
     DevBuf imp_as;                 // zk_import_asset_calls (import.cu): the hash table, references and grown slot table
     DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
@@ -107,6 +109,59 @@ struct zk_ctx {
     size_t pending_bytes = 0;      // result bytes of the MSM in flight (0 = none)
     uint8_t *h_pinned = nullptr;   // small pinned buffer for results
     size_t h_pinned_cap = 0;
+};
+
+// A host form's staging through ctx->io.  Each array is registered once: its host pointer, the device pointer to fill in,
+// its element count and its direction.  up() carves ctx->io in Carve's pieces, fills in every device pointer and copies
+// the in and in-out arrays up; down(), after the caller has enqueued its run, copies the out and in-out arrays back.  Both
+// enqueue on ctx->stream and neither synchronises.  A NULL host pointer gets a NULL device pointer, no space and no
+// copy; a count of 0 gets a valid device pointer and no copy.  An output registered with rows and width comes down for
+// *rows rows of width elements (*rows read by down(), at most count elements): a table whose final size is known only
+// after the run.
+struct Stage {
+    template <class T, class D> void in(const T *h, D *&d, size_t count) { add(h, d, count, true, false, nullptr, 1); }
+    template <class T, class D> void out(T *h, D *&d, size_t count, const size_t *rows = nullptr, size_t width = 1) {
+        add(h, d, count, false, true, rows, width);
+    }
+    template <class T, class D> void inout(T *h, D *&d, size_t count) { add(h, d, count, true, true, nullptr, 1); }
+
+    int up(zk_ctx *ctx) {
+        Carve sizing;
+        for (const Item &it : items) sizing.take<uint8_t>(it.elem * it.count);
+        ZK_TRY(ctx->io.reserve(sizing.off ? sizing.off : 1));     // 1: a buffer to point into when every count is 0
+        Carve c{ctx->io.as<uint8_t>(), 0};
+        for (Item &it : items) {
+            it.dev = c.take<uint8_t>(it.elem * it.count);
+            it.set(it.slot, it.dev);
+            if (it.to_dev && it.count) ZK_CUDA(cudaMemcpyAsync(it.dev, it.host, it.elem * it.count, cudaMemcpyHostToDevice, ctx->stream));
+        }
+        return ZK_OK;
+    }
+    int down(zk_ctx *ctx) {
+        for (const Item &it : items) {
+            const size_t n = it.rows && *it.rows * it.width < it.count ? *it.rows * it.width : it.count;
+            if (it.to_host && n) ZK_CUDA(cudaMemcpyAsync(it.host, it.dev, it.elem * n, cudaMemcpyDeviceToHost, ctx->stream));
+        }
+        return ZK_OK;
+    }
+
+  private:
+    struct Item {
+        void *host, *slot;
+        void (*set)(void *slot, uint8_t *dev);
+        uint8_t *dev;
+        size_t elem, count, width;
+        bool to_dev, to_host;
+        const size_t *rows;
+    };
+    std::vector<Item> items;
+    template <class T, class D> void add(const T *h, D *&d, size_t count, bool to_dev, bool to_host, const size_t *rows, size_t width) {
+        static_assert(std::is_same<typename std::remove_const<D>::type, T>::value, "a host array and its device copy have one element type");
+        d = nullptr;
+        if (h)
+            items.push_back({const_cast<T *>(h), &d, [](void *slot, uint8_t *dev) { *static_cast<D **>(slot) = reinterpret_cast<D *>(dev); },
+                             nullptr, sizeof(T), count, width, to_dev, to_host, rows});
+    }
 };
 
 struct zk_bases {

@@ -51,14 +51,15 @@ extern "C" int zk_jubjub_into_xy(zk_ctx *ctx, size_t n, const uint8_t *points, u
     if (!ctx || (n && (!points || !xy || !status))) { zk_set_error("zk_jubjub_into_xy: NULL argument"); return ZK_ERR_INVALID; }
     if (!n) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    const size_t in_bytes = 32 * n, xy_bytes = 64 * n;
-    ZK_TRY(ctx->v_io.reserve(in_bytes + xy_bytes + n));
-    uint8_t *d_in = ctx->v_io.as<uint8_t>(), *d_xy = d_in + in_bytes, *d_st = d_xy + xy_bytes;
-    ZK_CUDA(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    zk_launch_jubjub_into_xy(ctx->stream, d_in, n, reinterpret_cast<uint64_t *>(d_xy), d_st);
+    const uint8_t *d_in;
+    uint64_t *d_xy;
+    uint8_t *d_st;
+    Stage io;
+    io.in(points, d_in, 32 * n); io.out(xy, d_xy, 8 * n); io.out(status, d_st, n);
+    ZK_TRY(io.up(ctx));
+    zk_launch_jubjub_into_xy(ctx->stream, d_in, n, d_xy, d_st);
     ZK_CUDA(cudaGetLastError());
-    ZK_CUDA(cudaMemcpyAsync(xy, d_xy, xy_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(status, d_st, n, cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_TRY(io.down(ctx));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     return ZK_OK;
 }

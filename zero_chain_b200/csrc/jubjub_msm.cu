@@ -433,21 +433,19 @@ extern "C" int zk_redjubjub_batch_verify(zk_ctx *ctx, size_t n, const uint8_t *v
         return ZK_OK;
     }
     ZK_TRY(zk_use_device(ctx));
-    const uint64_t base = msg_off[0];
-    const size_t off_bytes = 8 * (n + 1), msg_bytes = msg_off[n] - base;
-    ZK_TRY(ctx->v_io.reserve(off_bytes + 8 + 128 * n + 1 + msg_bytes));
-    uint8_t *d_off = ctx->v_io.as<uint8_t>(), *d_first = d_off + off_bytes, *d_zs = d_first + 8, *d_vks = d_zs + 32 * n, *d_sigs = d_vks + 32 * n,
-            *d_ver = d_sigs + 64 * n, *d_msgs = d_ver + 1;
-    ZK_CUDA(cudaMemcpyAsync(d_off, msg_off, off_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d_zs, zs, 32 * n, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d_vks, vks, 32 * n, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d_sigs, sigs, 64 * n, cudaMemcpyHostToDevice, ctx->stream));
-    if (msg_bytes) ZK_CUDA(cudaMemcpyAsync(d_msgs, msgs + base, msg_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_TRY(rj_batch_launch(ctx, n, d_vks, d_sigs, d_msgs, reinterpret_cast<const uint64_t *>(d_off), base, d_zs, d_ver,
-                           reinterpret_cast<uint64_t *>(d_first)));
-    uint64_t fb = 0;
-    ZK_CUDA(cudaMemcpyAsync(verdict, d_ver, 1, cudaMemcpyDeviceToHost, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(&fb, d_first, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint64_t base = msg_off[0];       // the messages go up from msgs[base]; the kernel subtracts base from each offset
+    uint64_t fb = 0;                        // first_bad may be NULL; the device writes it all the same
+    const uint8_t *d_zs, *d_vks, *d_sigs, *d_msgs;
+    const uint64_t *d_off;
+    uint8_t *d_ver;
+    uint64_t *d_first;
+    Stage io;
+    io.in(msg_off, d_off, n + 1); io.in(zs, d_zs, 32 * n); io.in(vks, d_vks, 32 * n); io.in(sigs, d_sigs, 64 * n);
+    io.in(msgs + base, d_msgs, msg_off[n] - base);
+    io.out(verdict, d_ver, 1); io.out(&fb, d_first, 1);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(rj_batch_launch(ctx, n, d_vks, d_sigs, d_msgs, d_off, base, d_zs, d_ver, d_first));
+    ZK_TRY(io.down(ctx));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     if (first_bad) *first_bad = fb;
     return ZK_OK;

@@ -415,14 +415,13 @@ extern "C" int zk_groth16_verify_points_batch(zk_ctx *ctx, const zk_pvk *k, size
     }
     if (!n) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    const size_t pt_bytes = n * n_points * 32;
-    ZK_TRY(ctx->v_io.reserve(n * 192 + pt_bytes + n + 64));
-    uint8_t *d = ctx->v_io.as<uint8_t>();
-    uint8_t *d_pts = d + ((n * 192 + 15) & ~(size_t)15), *d_out = d_pts + pt_bytes;
-    ZK_CUDA(cudaMemcpyAsync(d, proofs, n * 192, cudaMemcpyHostToDevice, ctx->stream));
-    if (pt_bytes) ZK_CUDA(cudaMemcpyAsync(d_pts, points, pt_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_TRY(zk_groth16_verify_points_batch_device(ctx, k, n, d, d_pts, n_points, d_out));
-    ZK_CUDA(cudaMemcpyAsync(verdicts, d_out, n, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint8_t *d_proofs, *d_pts;
+    uint8_t *d_out;
+    Stage io;
+    io.in(proofs, d_proofs, 192 * n); io.in(points, d_pts, 32 * n * n_points); io.out(verdicts, d_out, n);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(zk_groth16_verify_points_batch_device(ctx, k, n, d_proofs, d_pts, n_points, d_out));
+    ZK_TRY(io.down(ctx));
     return zk_check_err_flag(ctx);      // synchronises
 }
 
@@ -435,14 +434,14 @@ extern "C" int zk_groth16_verify_batch(zk_ctx *ctx, const zk_pvk *k, size_t n, c
     }
     if (!n) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    size_t in_bytes = n * n_inputs * 32;
-    ZK_TRY(ctx->v_io.reserve(n * 192 + in_bytes + n + 64));
-    uint8_t *d = ctx->v_io.as<uint8_t>();
-    uint8_t *d_in = d + ((n * 192 + 15) & ~(size_t)15), *d_out = d_in + in_bytes;
-    ZK_CUDA(cudaMemcpyAsync(d, proofs, n * 192, cudaMemcpyHostToDevice, ctx->stream));
-    if (in_bytes) ZK_CUDA(cudaMemcpyAsync(d_in, inputs, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_TRY(zk_groth16_verify_batch_device(ctx, k, n, d, (const uint64_t *)d_in, n_inputs, d_out));
-    ZK_CUDA(cudaMemcpyAsync(verdicts, d_out, n, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint8_t *d_proofs;
+    const uint64_t *d_in;
+    uint8_t *d_out;
+    Stage io;
+    io.in(proofs, d_proofs, 192 * n); io.in(inputs, d_in, 4 * n * n_inputs); io.out(verdicts, d_out, n);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(zk_groth16_verify_batch_device(ctx, k, n, d_proofs, d_in, n_inputs, d_out));
+    ZK_TRY(io.down(ctx));
     return zk_check_err_flag(ctx);      // synchronises; ZK_ERR_NOT_CANONICAL if an input was >= r
 }
 
@@ -451,22 +450,23 @@ extern "C" int zk_pairing_batch(zk_ctx *ctx, size_t n, const uint8_t *g1, const 
     if (!ctx || (n && (!g1 || !g2 || !out))) { zk_set_error("zk_pairing_batch: NULL argument"); return ZK_ERR_INVALID; }
     if (!n) return ZK_OK;
     ZK_TRY(zk_use_device(ctx));
-    ZK_TRY(ctx->v_io.reserve(n * (96 + 192 + 576)));
+    const uint8_t *d1, *d2;
+    uint8_t *dout;
+    Stage io;
+    io.in(g1, d1, 96 * n); io.in(g2, d2, 192 * n); io.out(out, dout, 576 * n);
     ZK_TRY(ctx->v_pts.reserve(n * (sizeof(G1A) + sizeof(G2A))));
     ZK_TRY(ctx->v_f.reserve(n * sizeof(Fq12)));
-    uint8_t *d1 = ctx->v_io.as<uint8_t>(), *d2 = d1 + n * 96, *dout = d2 + n * 192;
+    ZK_TRY(io.up(ctx));
     G1A *p = ctx->v_pts.as<G1A>();
     G2A *q = (G2A *)(p + n);
     int *err = ctx->d_err + 1;
-    ZK_CUDA(cudaMemcpyAsync(d1, g1, n * 96, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d2, g2, n * 192, cudaMemcpyHostToDevice, ctx->stream));
     zkcodec::k_decode_uncompressed<Fq><<<grid(n, 128), 128, 0, ctx->stream>>>(d1, n, 1, 0, p, err);
     zkcodec::k_decode_uncompressed<Fq2><<<grid(n, 128), 128, 0, ctx->stream>>>(d2, n, 1, 0, q, err);
     ZK_TRY(zk_check_err_flag(ctx));
     ZK_TRY(pairing_device(ctx, p, q, n, ctx->v_f.as<Fq12>()));
     k_fq_store_be<<<grid(n * 12, 128), 128, 0, ctx->stream>>>((const Fq *)ctx->v_f.p, n * 12, dout);
     ZK_CUDA(cudaGetLastError());
-    ZK_CUDA(cudaMemcpyAsync(out, dout, n * 576, cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_TRY(io.down(ctx));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     return ZK_OK;
 }

@@ -63,18 +63,17 @@ extern "C" int zk_redjubjub_verify_batch(zk_ctx *ctx, size_t n, const uint8_t *v
             return ZK_ERR_INVALID;
         }
     ZK_TRY(zk_use_device(ctx));
-    const uint64_t base = msg_off[0];
-    const size_t off_bytes = 8 * (n + 1), msg_bytes = msg_off[n] - base;
-    ZK_TRY(ctx->v_io.reserve(off_bytes + 97 * n + msg_bytes));
-    uint8_t *d_off = ctx->v_io.as<uint8_t>(), *d_vks = d_off + off_bytes, *d_sigs = d_vks + 32 * n, *d_ver = d_sigs + 64 * n,
-            *d_msgs = d_ver + n;
-    ZK_CUDA(cudaMemcpyAsync(d_off, msg_off, off_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d_vks, vks, 32 * n, cudaMemcpyHostToDevice, ctx->stream));
-    ZK_CUDA(cudaMemcpyAsync(d_sigs, sigs, 64 * n, cudaMemcpyHostToDevice, ctx->stream));
-    if (msg_bytes) ZK_CUDA(cudaMemcpyAsync(d_msgs, msgs + base, msg_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    launch_verify(ctx, n, d_vks, d_sigs, d_msgs, reinterpret_cast<const uint64_t *>(d_off), base, d_ver);
+    const uint64_t base = msg_off[0];       // the messages go up from msgs[base]; the kernel subtracts base from each offset
+    const uint8_t *d_vks, *d_sigs, *d_msgs;
+    const uint64_t *d_off;
+    uint8_t *d_ver;
+    Stage io;
+    io.in(msg_off, d_off, n + 1); io.in(vks, d_vks, 32 * n); io.in(sigs, d_sigs, 64 * n); io.in(msgs + base, d_msgs, msg_off[n] - base);
+    io.out(verdicts, d_ver, n);
+    ZK_TRY(io.up(ctx));
+    launch_verify(ctx, n, d_vks, d_sigs, d_msgs, d_off, base, d_ver);
     ZK_CUDA(cudaGetLastError());
-    ZK_CUDA(cudaMemcpyAsync(verdicts, d_ver, n, cudaMemcpyDeviceToHost, ctx->stream));
+    ZK_TRY(io.down(ctx));
     ZK_CUDA(cudaStreamSynchronize(ctx->stream));
     return ZK_OK;
 }
