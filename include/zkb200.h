@@ -309,6 +309,50 @@ int zk_elgamal_decrypt_batch(zk_ctx *ctx, size_t n, const uint8_t *dks, const ui
 /* the same with device pointers (d_values 4-byte aligned); asynchronous on the context's stream */
 int zk_elgamal_decrypt_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_dks, const uint8_t *d_cts, const uint8_t *d_pending,
                                     uint32_t *d_values, uint8_t *d_status);
+/* ---- building confidential transfers (what zface's gen_proof / gen_xt run around the proof) -----------------------
+ * All with the Diversifier generator P_G; scalars are 32 B little-endian Fs, points 32 B Point::write encodings.
+ * SpendingKey::from_seed -> ProofGenerationKey -> DecryptionKey -> EncryptionKey (core/keys/src/lib.rs:64-71, 167-199) for n
+ * seeds of any length: seed i = seeds[seed_off[i] .. seed_off[i+1]), as the messages of zk_redjubjub_verify_batch.
+ * sks / dks / eks: n * 32 B.  ZK_ERR_INVALID for a NULL pointer with n > 0, or for offsets that decrease. */
+int zk_keys_from_seed_batch(zk_ctx *ctx, size_t n, const uint8_t *seeds, const uint64_t *seed_off, uint8_t *sks, uint8_t *dks,
+                            uint8_t *eks);
+/* the same with device pointers; asynchronous on the context's stream.  The offsets are not checked: they must not decrease. */
+int zk_keys_from_seed_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_seeds, const uint64_t *d_seed_off, uint8_t *d_sks,
+                                   uint8_t *d_dks, uint8_t *d_eks);
+/* GEpoch::group_hash(epochs[i]) (core/primitives/src/g_epoch.rs:102-145) for n epochs: g_epochs = n * 32 B.  ZK_ERR_DECODE,
+ * naming the epoch, when no tag byte below 255 gives a point (the reference asserts there); ZK_ERR_INVALID for NULL. */
+int zk_g_epoch_batch(zk_ctx *ctx, size_t n, const uint32_t *epochs, uint8_t *g_epochs);
+/* the same with device pointers; asynchronous.  A row whose hash would need tag byte 255 is left as 32 bytes of 0xff. */
+int zk_g_epoch_batch_device(zk_ctx *ctx, size_t n, const uint32_t *d_epochs, uint8_t *d_g_epochs);
+/* The fields of n confidential transfers: MultiCiphertexts::<Confidential>::encrypt (core/crypto/src/elgamal.rs:48-66) and
+ * ProofContext's rvk and nonce, from the sender's sk (n * 32 B), the recipient's encryption key (n * 32 B), amount and fee
+ * (n uint32 each), the ElGamal randomness r and the re-randomizer alpha (n * 32 B each) and the call's g_epoch (32 B).
+ * fields: n * 288 B, per row the 9 points in the order of groth16.ConfidentialTx's constructor: address_sender (= ek_s),
+ *   address_recipient (copied), amount_sender = amount P_G + r ek_s, amount_recipient = amount P_G + r ek_r,
+ *   fee_sender = fee P_G + r ek_s, randomness = r P_G, rvk = pgk + alpha P_G, g_epoch (copied), nonce = dk g_epoch.
+ * rsks: n * 32 B, sk + alpha mod r_J; dks: n * 32 B, the sender's decryption key.
+ * status[i]: 0, or the zk_jubjub_into_xy code (1 / 2 / 3) of a recipient key that fails EncryptionKey::read
+ *   (Point::read + as_prime_order); that row's fields, rsk and dk are zero and the other rows are unaffected.
+ * ZK_ERR_NOT_CANONICAL (zk_last_error names the array and the lowest index) for an sk, r or alpha >= r_J; ZK_ERR_DECODE
+ * for a g_epoch that fails Point::read or is not of prime order (the outputs are then undefined); ZK_ERR_INVALID for NULL. */
+int zk_confidential_fields_batch(zk_ctx *ctx, size_t n, const uint8_t *sks, const uint8_t *eks_recipient, const uint32_t *amounts,
+                                 const uint32_t *fees, const uint8_t *rs, const uint8_t *alphas, const uint8_t *g_epoch, uint8_t *fields,
+                                 uint8_t *rsks, uint8_t *dks, uint8_t *status);
+/* the same with device pointers (d_g_epoch: 32 B on the device); asynchronous on the context's stream.  The next zk_ctx_sync
+ * reports ZK_ERR_NOT_CANONICAL (a row with an sk, r or alpha >= r_J is left unwritten) or ZK_ERR_DECODE (g_epoch). */
+int zk_confidential_fields_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_sks, const uint8_t *d_eks_recipient,
+                                        const uint32_t *d_amounts, const uint32_t *d_fees, const uint8_t *d_rs, const uint8_t *d_alphas,
+                                        const uint8_t *d_g_epoch, uint8_t *d_fields, uint8_t *d_rsks, uint8_t *d_dks, uint8_t *d_status);
+/* PrivateKey::sign(msg, rng, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:73-103) for n messages, with the
+ * 80 random bytes T of each signature supplied by the caller: ts = n * 80 B.  sks: n * 32 B; msgs / msg_off exactly as
+ * zk_redjubjub_verify_batch; sigs: n * 64 B (rbar | sbar).  ZK_ERR_NOT_CANONICAL (naming the lowest index) for an
+ * sk >= r_J; ZK_ERR_INVALID for NULL, or for offsets that decrease. */
+int zk_redjubjub_sign_batch(zk_ctx *ctx, size_t n, const uint8_t *sks, const uint8_t *ts, const uint8_t *msgs, const uint64_t *msg_off,
+                            uint8_t *sigs);
+/* the same with device pointers; asynchronous.  The offsets are not checked; an sk >= r_J leaves its signature unwritten
+ * and the next zk_ctx_sync reports ZK_ERR_NOT_CANONICAL. */
+int zk_redjubjub_sign_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_sks, const uint8_t *d_ts, const uint8_t *d_msgs,
+                                   const uint64_t *d_msg_off, uint8_t *d_sigs);
 /* ---- confidential-transfer balance updates of one block (what modules/encrypted-balances runs around each proof) ------
  * rollover + sub_enc_balance + add_pending_transfer (modules/encrypted-balances/src/lib.rs:25-96, 133-222) for n_tx
  * transactions, in order, over a table of n_accounts accounts.

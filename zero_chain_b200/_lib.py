@@ -77,6 +77,14 @@ SIGNATURES = {
     "zk_redjubjub_batch_verify_device": (i32, [vp, sz, vp, vp, vp, vp, vp, vp, vp]),
     "zk_elgamal_decrypt_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_elgamal_decrypt_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_keys_from_seed_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_keys_from_seed_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_g_epoch_batch": (i32, [vp, sz, vp, vp]),
+    "zk_g_epoch_batch_device": (i32, [vp, sz, vp, vp]),
+    "zk_confidential_fields_batch": (i32, [vp, sz] + [vp] * 11),
+    "zk_confidential_fields_batch_device": (i32, [vp, sz] + [vp] * 11),
+    "zk_redjubjub_sign_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_redjubjub_sign_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_balances_confidential_block": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_confidential_block_device": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_anonymous_block": (i32, [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -548,6 +548,109 @@ def elgamal_decrypt_device(ctx: Context, n: int, d_dks_ptr: int, d_cts_ptr: int,
                                                    C.c_void_p(d_status_ptr)))
 
 
+# ---- building confidential transfers (zface's gen_proof / gen_xt around the proof) ----------------------------------------
+# zk_confidential_fields_batch: the 9 points of a row in ConfidentialTx's constructor order
+CONFIDENTIAL_FIELDS = ("address_sender", "address_recipient", "amount_sender", "amount_recipient", "fee_sender", "randomness", "rvk",
+                       "g_epoch", "nonce")
+
+
+def _buf(b: bytes):
+    return np.frombuffer(b, np.uint8) if b else np.zeros(1, np.uint8)
+
+
+def _scalars(v, n: int) -> bytes:
+    """n 32-byte little-endian scalars from ints or byte strings (or one concatenation)"""
+    if not isinstance(v, (bytes, bytearray, memoryview)):
+        v = [s.to_bytes(32, "little") if isinstance(s, int) else s for s in v]
+    b = _cat(v, 32)
+    assert len(b) == 32 * n, (len(b), n)
+    return b
+
+
+def _rows(out: np.ndarray, size: int, n: int) -> list:
+    return [out[size * i:size * (i + 1)].tobytes() for i in range(n)]
+
+
+def keys_from_seed(ctx: Context, seeds):
+    """SpendingKey::from_seed -> DecryptionKey -> EncryptionKey (core/keys/src/lib.rs) of each seed (byte strings of any
+    length).  Returns (sks, dks, eks): lists of 32-byte values."""
+    n = len(seeds)
+    sk, dk, ek = (np.zeros(max(32 * n, 1), np.uint8) for _ in range(3))
+    _ck(_lib.lib().zk_keys_from_seed_batch(ctx._h, n, _p(_buf(b"".join(bytes(s) for s in seeds))), _p(message_offsets(seeds)), _p(sk), _p(dk),
+                                           _p(ek)))
+    return _rows(sk, 32, n), _rows(dk, 32, n), _rows(ek, 32, n)
+
+
+def keys_from_seed_device(ctx: Context, n: int, d_seeds_ptr: int, d_seed_off_ptr: int, d_sks_ptr: int, d_dks_ptr: int, d_eks_ptr: int):
+    """The same on device pointers (d_seed_off: n + 1 uint64 offsets), asynchronous on the context's stream."""
+    _ck(_lib.lib().zk_keys_from_seed_batch_device(ctx._h, n, C.c_void_p(d_seeds_ptr), C.c_void_p(d_seed_off_ptr), C.c_void_p(d_sks_ptr),
+                                                  C.c_void_p(d_dks_ptr), C.c_void_p(d_eks_ptr)))
+
+
+def g_epoch(ctx: Context, epochs) -> list:
+    """GEpoch::group_hash(epoch) (core/primitives/src/g_epoch.rs:102-145) of each epoch: a list of 32-byte encodings."""
+    n = len(epochs)
+    ep = np.ascontiguousarray(epochs, np.uint32) if n else np.zeros(1, np.uint32)
+    out = np.zeros(max(32 * n, 1), np.uint8)
+    _ck(_lib.lib().zk_g_epoch_batch(ctx._h, n, _p(ep), _p(out)))
+    return _rows(out, 32, n)
+
+
+def g_epoch_device(ctx: Context, n: int, d_epochs_ptr: int, d_g_epochs_ptr: int):
+    """The same on device pointers (d_epochs: n uint32), asynchronous on the context's stream."""
+    _ck(_lib.lib().zk_g_epoch_batch_device(ctx._h, n, C.c_void_p(d_epochs_ptr), C.c_void_p(d_g_epochs_ptr)))
+
+
+def confidential_fields(ctx: Context, sks, eks_recipient, amounts, fees, rs, alphas, g_epoch_enc):
+    """The ciphertexts, rvk and nonce of n confidential transfers (MultiCiphertexts::<Confidential>::encrypt and ProofContext):
+    sks / rs / alphas are scalars < r_J (ints or 32 bytes), eks_recipient 32-byte keys, amounts / fees uint32, g_epoch_enc
+    the call's 32-byte g_epoch.  Returns (fields, rsks, dks, status): fields[i] is a dict of the CONFIDENTIAL_FIELDS
+    (ConfidentialTx(sender, recipient, **fields[i]) builds the extrinsic), rsks / dks 32-byte values, status the
+    zk_jubjub_into_xy code of each recipient key (0: ok; otherwise the row is zero)."""
+    n = len(amounts)
+    sk, r, al = _scalars(sks, n), _scalars(rs, n), _scalars(alphas, n)
+    ek = _cat(eks_recipient, 32)
+    assert len(ek) == 32 * n and len(fees) == n
+    am = np.ascontiguousarray(amounts, np.uint32) if n else np.zeros(1, np.uint32)
+    fe = np.ascontiguousarray(fees, np.uint32) if n else np.zeros(1, np.uint32)
+    f = np.zeros(max(288 * n, 1), np.uint8)
+    rsk, dk, st = np.zeros(max(32 * n, 1), np.uint8), np.zeros(max(32 * n, 1), np.uint8), np.zeros(max(n, 1), np.uint8)
+    _ck(_lib.lib().zk_confidential_fields_batch(ctx._h, n, _p(_buf(sk)), _p(_buf(ek)), _p(am), _p(fe), _p(_buf(r)), _p(_buf(al)),
+                                                _p(_buf(_pt32(g_epoch_enc))), _p(f), _p(rsk), _p(dk), _p(st)))
+    fields = [dict(zip(CONFIDENTIAL_FIELDS, _rows(f[288 * i:288 * (i + 1)], 32, 9))) for i in range(n)]
+    return fields, _rows(rsk, 32, n), _rows(dk, 32, n), [int(s) for s in st[:n]]
+
+
+def confidential_fields_device(ctx: Context, n: int, d_sks_ptr: int, d_eks_recipient_ptr: int, d_amounts_ptr: int, d_fees_ptr: int,
+                               d_rs_ptr: int, d_alphas_ptr: int, d_g_epoch_ptr: int, d_fields_ptr: int, d_rsks_ptr: int, d_dks_ptr: int,
+                               d_status_ptr: int):
+    """The same on device pointers (d_amounts / d_fees: n uint32; d_fields: n * 288 bytes), asynchronous on the context's
+    stream; ctx.sync() raises ZK_ERR_NOT_CANONICAL or ZK_ERR_DECODE (g_epoch)."""
+    _ck(_lib.lib().zk_confidential_fields_batch_device(ctx._h, n, *(C.c_void_p(p) for p in (
+        d_sks_ptr, d_eks_recipient_ptr, d_amounts_ptr, d_fees_ptr, d_rs_ptr, d_alphas_ptr, d_g_epoch_ptr, d_fields_ptr, d_rsks_ptr,
+        d_dks_ptr, d_status_ptr))))
+
+
+def redjubjub_sign(ctx: Context, sks, msgs, ts) -> list:
+    """PrivateKey::sign(msg, rng, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:73-103) of each message, with
+    the 80 bytes ts[i] in place of the RNG's output (draw them with secrets.token_bytes(80)).  sks: scalars < r_J (ints or
+    32 bytes).  Returns the 64-byte signatures (rbar | sbar)."""
+    n = len(msgs)
+    sk, t = _scalars(sks, n), _cat(ts, 80)
+    assert len(t) == 80 * n
+    out = np.zeros(max(64 * n, 1), np.uint8)
+    _ck(_lib.lib().zk_redjubjub_sign_batch(ctx._h, n, _p(_buf(sk)), _p(_buf(t)), _p(_buf(b"".join(bytes(m) for m in msgs))),
+                                           _p(message_offsets(msgs)), _p(out)))
+    return _rows(out, 64, n)
+
+
+def redjubjub_sign_device(ctx: Context, n: int, d_sks_ptr: int, d_ts_ptr: int, d_msgs_ptr: int, d_msg_off_ptr: int, d_sigs_ptr: int):
+    """The same on device pointers (d_ts: n * 80 bytes; d_msg_off: n + 1 uint64 offsets), asynchronous on the context's
+    stream."""
+    _ck(_lib.lib().zk_redjubjub_sign_batch_device(ctx._h, n, C.c_void_p(d_sks_ptr), C.c_void_p(d_ts_ptr), C.c_void_p(d_msgs_ptr),
+                                                  C.c_void_p(d_msg_off_ptr), C.c_void_p(d_sigs_ptr)))
+
+
 # ---- confidential-transfer balance updates of one block (modules/encrypted-balances/src/lib.rs:25-96, 133-222) ----------
 # account flags and zk_balances_confidential_block statuses
 ACCOUNT_BALANCE, ACCOUNT_PENDING, ACCOUNT_DUE = 1, 2, 4
