@@ -343,6 +343,35 @@ int zk_confidential_fields_batch(zk_ctx *ctx, size_t n, const uint8_t *sks, cons
 int zk_confidential_fields_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_sks, const uint8_t *d_eks_recipient,
                                         const uint32_t *d_amounts, const uint32_t *d_fees, const uint8_t *d_rs, const uint8_t *d_alphas,
                                         const uint8_t *d_g_epoch, uint8_t *d_fields, uint8_t *d_rsks, uint8_t *d_dks, uint8_t *d_status);
+/* The fields of n anonymous transfers: MultiCiphertexts::<Anonymous>::encrypt (core/proofs/src/crypto_components.rs:168-216)
+ * placed in ring order as gen_proof places them (core/proofs/src/anonymous.rs:97-145), with ProofContext's rvk and nonce.
+ * keys: a table of n_keys 32-byte encryption keys (a wallet's EncKeySet, or a block's account table); NULL only when
+ *   n_keys = 0.  Each key an in-range ring index names is read (EncryptionKey::read) once per call; the others are not read.
+ * rings: n * 11 uint32 indices into keys, in MultiEncKeys order: [0] the recipient, [1..11) the ten decoys in order.
+ * positions: n * 2 bytes, s_index then t_index.  amounts: n uint32 (there is no fee).  sks, rs, alphas: n * 32 B of Fs
+ *   (the sender's spending key, the ElGamal randomness r, the re-randomizer alpha).  g_epoch: 32 B.
+ * fields: n * 864 B, per row 27 points in the argument order of groth16.AnonymousTx after the member indices:
+ *   enc_keys[12] | left_ciphertexts[12] | right_ciphertext | rvk | nonce.  The sender sits at s, the recipient at t, and the
+ *   decoys fill the other ten positions in their order.  enc_keys[s] = ek_s = dk P_G, enc_keys at the others are the
+ *   table's bytes copied; left_ciphertexts[s] = -amount P_G + r ek_s (neg_encrypt), [t] = amount P_G + r ek_t (encrypt),
+ *   a decoy's = r ek_d (encrypt of 0); right_ciphertext = r P_G, rvk = pgk + alpha P_G, nonce = dk g_epoch.
+ * rsks: n * 32 B, sk + alpha mod r_J; dks: n * 32 B, the sender's decryption key.
+ * status[i]: 0 built; 5 s >= 12, t >= 12 or s = t; 4 a ring index >= n_keys; else 1 / 2 / 3, the zk_jubjub_into_xy code of
+ *   the row's first key, in MultiEncKeys order, that fails EncryptionKey::read.  5 comes before 4 and 4 before the key
+ *   codes.  A row with a non-zero status gets all-zero fields, rsk and dk; the other rows are unaffected.
+ * ZK_ERR_NOT_CANONICAL (zk_last_error names the array and the lowest index) for an sk, r or alpha >= r_J; ZK_ERR_DECODE
+ * for a g_epoch that fails Point::read or is not of prime order (the outputs are then undefined); ZK_ERR_INVALID for NULL,
+ * and for n above 2^22 or n_keys above 2^24. */
+int zk_anonymous_fields_batch(zk_ctx *ctx, size_t n_keys, const uint8_t *keys, size_t n, const uint8_t *sks, const uint32_t *rings,
+                              const uint8_t *positions, const uint32_t *amounts, const uint8_t *rs, const uint8_t *alphas,
+                              const uint8_t *g_epoch, uint8_t *fields, uint8_t *rsks, uint8_t *dks, uint8_t *status);
+/* the same with device pointers (d_rings and d_amounts 4-byte aligned, d_g_epoch: 32 B on the device); asynchronous on the
+ * context's stream.  The next zk_ctx_sync reports ZK_ERR_NOT_CANONICAL (a row with an sk, r or alpha >= r_J is left
+ * unwritten) or ZK_ERR_DECODE (g_epoch). */
+int zk_anonymous_fields_batch_device(zk_ctx *ctx, size_t n_keys, const uint8_t *d_keys, size_t n, const uint8_t *d_sks,
+                                     const uint32_t *d_rings, const uint8_t *d_positions, const uint32_t *d_amounts, const uint8_t *d_rs,
+                                     const uint8_t *d_alphas, const uint8_t *d_g_epoch, uint8_t *d_fields, uint8_t *d_rsks,
+                                     uint8_t *d_dks, uint8_t *d_status);
 /* PrivateKey::sign(msg, rng, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:73-103) for n messages, with the
  * 80 random bytes T of each signature supplied by the caller: ts = n * 80 B.  sks: n * 32 B; msgs / msg_off exactly as
  * zk_redjubjub_verify_batch; sigs: n * 64 B (rbar | sbar).  ZK_ERR_NOT_CANONICAL (naming the lowest index) for an

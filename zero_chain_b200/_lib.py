@@ -83,6 +83,8 @@ SIGNATURES = {
     "zk_g_epoch_batch_device": (i32, [vp, sz, vp, vp]),
     "zk_confidential_fields_batch": (i32, [vp, sz] + [vp] * 11),
     "zk_confidential_fields_batch_device": (i32, [vp, sz] + [vp] * 11),
+    "zk_anonymous_fields_batch": (i32, [vp, sz, vp, sz] + [vp] * 11),
+    "zk_anonymous_fields_batch_device": (i32, [vp, sz, vp, sz] + [vp] * 11),
     "zk_redjubjub_sign_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_redjubjub_sign_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_balances_confidential_block": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -1,7 +1,9 @@
 // Building confidential transfers on the device (tx_build.cuh): zk_keys_from_seed_batch, zk_g_epoch_batch,
 // zk_confidential_fields_batch and zk_redjubjub_sign_batch, each with its _device form.  One thread per row, everything
 // in registers; the fields call parks each row's seven points in a workspace of the context between its two passes and
-// first builds the window table of the call's g_epoch with one thread per entry.
+// first builds the window table of the call's g_epoch with one thread per entry.  zk_anonymous_fields_batch decodes each key
+// its rings name once, then runs a pass per row and a pass per (row, ring entry), so a row's 11 variable-base products
+// spread over 11 threads.
 //
 // Like redjubjub.cu, the translation unit holds only Fr / Fs arithmetic and is compiled with everything inlined (ZK_HOT).
 #define ZK_HOT 1
@@ -100,6 +102,71 @@ static __global__ void __launch_bounds__(TT) k_tb_sign(size_t n, const uint8_t *
         const uint64_t o0 = off[i] - base, o1 = off[i + 1] - base;
         redjubjub_sign(fs_words(sk), t, msgs + o0, o1 - o0, sig);
         store_le_words(sigs + 64 * i, sig, 16);
+    }
+}
+
+// ---- zk_anonymous_fields_batch: the key table, then the row pass, then the left pass -------------------------------------
+// one thread per ring index: flags each key an in-range index names (named[] zeroed before)
+static __global__ void __launch_bounds__(TT) k_tb_anon_named(size_t m, const uint32_t *__restrict__ rings, size_t n_keys,
+                                                             uint8_t *__restrict__ named) {
+    TB_ROWS(k, m) {
+        const uint32_t idx = rings[k];
+        if (idx < n_keys) named[idx] = 1;
+    }
+}
+
+// one thread per key: a named key is read once, whatever number of rows name it; the others are left alone
+static __global__ void __launch_bounds__(TT) k_tb_anon_keys(size_t n_keys, const uint8_t *__restrict__ keys, const uint8_t *__restrict__ named,
+                                                            uint32_t *__restrict__ niels, uint8_t *__restrict__ key_status) {
+    TB_ROWS(k, n_keys) {
+        if (!named[k]) continue;
+        uint32_t w[8];
+        load_le_words(keys + 32 * k, w, 8);
+        key_status[k] = (uint8_t)anon_key_entry(w, niels + TB_ENTRY_WORDS * k);
+    }
+}
+
+static __device__ __forceinline__ bool anon_canonical(size_t i, const uint8_t *sks, const uint8_t *rs, const uint8_t *alphas, uint32_t *sk,
+                                                      uint32_t *r, uint32_t *al) {
+    load_le_words(sks + 32 * i, sk, 8); load_le_words(rs + 32 * i, r, 8); load_le_words(alphas + 32 * i, al, 8);
+    return Fs::canonical_lt_mod(fs_words(sk)) && Fs::canonical_lt_mod(fs_words(r)) && Fs::canonical_lt_mod(fs_words(al));
+}
+
+static __global__ void __launch_bounds__(TT) k_tb_anon_rows(size_t n, const uint8_t *__restrict__ sks, const uint32_t *__restrict__ rings,
+                                                            const uint8_t *__restrict__ positions, const uint32_t *__restrict__ amounts,
+                                                            const uint8_t *__restrict__ rs, const uint8_t *__restrict__ alphas, size_t n_keys,
+                                                            const uint8_t *__restrict__ key_status, const uint32_t *__restrict__ table,
+                                                            uint32_t *__restrict__ scratch, uint8_t *__restrict__ fields,
+                                                            uint8_t *__restrict__ rsks, uint8_t *__restrict__ dks, uint8_t *__restrict__ status,
+                                                            int *not_canonical) {
+    TB_ROWS(i, n) {
+        uint32_t sk[8], r[8], al[8];
+        if (!anon_canonical(i, sks, rs, alphas, sk, r, al)) {
+            atomicExch(not_canonical, 1);
+            continue;
+        }
+        const int s = positions[2 * i], t = positions[2 * i + 1];
+        const int st = anon_status(s, t, rings + (size_t)TB_RING_IN * i, n_keys, key_status);
+        anonymous_row(st, s, sk, amounts[i], r, al, table, scratch + i, n, fields + 32 * TB_N_ANON_FIELDS * i, rsks + 32 * i, dks + 32 * i);
+        status[i] = (uint8_t)st;
+    }
+}
+
+// thread TB_RING_IN i + j: ring entry j of row i, so a row's entries run side by side; rows the row pass refused (status)
+// or skipped (a scalar >= r_J) are left as it left them
+static __global__ void __launch_bounds__(TT) k_tb_anon_lefts(size_t n, const uint8_t *__restrict__ keys, const uint32_t *__restrict__ rings,
+                                                             const uint8_t *__restrict__ positions, const uint32_t *__restrict__ amounts,
+                                                             const uint8_t *__restrict__ sks, const uint8_t *__restrict__ rs,
+                                                             const uint8_t *__restrict__ alphas, const uint32_t *__restrict__ niels,
+                                                             const uint8_t *__restrict__ status, uint8_t *__restrict__ fields) {
+    TB_ROWS(k, TB_RING_IN * n) {
+        const size_t i = k / TB_RING_IN;
+        const int j = (int)(k - TB_RING_IN * i);
+        uint32_t sk[8], r[8], al[8];
+        if (!anon_canonical(i, sks, rs, alphas, sk, r, al) || status[i] != JJ_OK) continue;
+        const size_t idx = rings[k];
+        anonymous_left(load_niels(niels + TB_ENTRY_WORDS * idx), keys + 32 * idx, j, anon_position(positions[2 * i], positions[2 * i + 1], j),
+                       amounts[i], r, fields + 32 * TB_N_ANON_FIELDS * i);
     }
 }
 
@@ -265,6 +332,93 @@ extern "C" int zk_confidential_fields_batch(zk_ctx *ctx, size_t n, const uint8_t
     io.out(fields, d_fields, 32 * TB_N_FIELDS * n); io.out(rsks, d_rsks, 32 * n); io.out(dks, d_dks, 32 * n); io.out(status, d_st, n);
     ZK_TRY(io.up(ctx));
     ZK_TRY(launch_fields(ctx, n, d_sks, d_eks, d_am, d_fee, d_rs, d_al, d_g, d_fields, d_rsks, d_dks, d_st));
+    ZK_TRY(io.down(ctx));
+    const int rc = zk_check_err_flag(ctx);   // synchronises the stream
+    if (rc == ZK_ERR_DECODE) zk_set_error("%s: g_epoch fails Point::read or is not of prime order", fn);
+    return rc;
+}
+
+// ---- zk_anonymous_fields_batch --------------------------------------------------------------------------------------------
+constexpr size_t TB_ANON_MAX_ROWS = (size_t)1 << 22, TB_ANON_MAX_KEYS = (size_t)1 << 24;
+
+static int check_anon_sizes(const char *fn, size_t n_keys, size_t n) {
+    if (n > TB_ANON_MAX_ROWS || n_keys > TB_ANON_MAX_KEYS) {
+        zk_set_error("%s: n = %zu, n_keys = %zu; at most 2^22 rows and 2^24 keys", fn, n, n_keys);
+        return ZK_ERR_INVALID;
+    }
+    return ZK_OK;
+}
+
+static int launch_anon(zk_ctx *ctx, size_t n_keys, const uint8_t *keys, size_t n, const uint8_t *sks, const uint32_t *rings,
+                       const uint8_t *positions, const uint32_t *amounts, const uint8_t *rs, const uint8_t *alphas, const uint8_t *g_epoch,
+                       uint8_t *fields, uint8_t *rsks, uint8_t *dks, uint8_t *status) {
+    Carve sizing;
+    sizing.take<uint32_t>(TB_TABLE_WORDS); sizing.take<uint32_t>(8 * TB_ANON_SCRATCH_SLOTS * n);
+    sizing.take<uint32_t>(TB_ENTRY_WORDS * n_keys); sizing.take<uint8_t>(n_keys); sizing.take<uint8_t>(n_keys);
+    ZK_TRY(ctx->tb.reserve(sizing.off));
+    Carve c{ctx->tb.as<uint8_t>(), 0};
+    uint32_t *table = c.take<uint32_t>(TB_TABLE_WORDS), *scratch = c.take<uint32_t>(8 * TB_ANON_SCRATCH_SLOTS * n);
+    uint32_t *niels = c.take<uint32_t>(TB_ENTRY_WORDS * n_keys);
+    uint8_t *named = c.take<uint8_t>(n_keys), *key_status = c.take<uint8_t>(n_keys);
+    k_tb_epoch_table<<<(TB_WINDOWS * TB_DIGITS + TT - 1) / TT, TT, 0, ctx->stream>>>(g_epoch, table, ctx->d_err + 1);
+    ZK_CUDA(cudaGetLastError());
+    if (n_keys) {
+        ZK_CUDA(cudaMemsetAsync(named, 0, n_keys, ctx->stream));
+        k_tb_anon_named<<<grid(ctx, TB_RING_IN * n), TT, 0, ctx->stream>>>(TB_RING_IN * n, rings, n_keys, named);
+        ZK_CUDA(cudaGetLastError());
+        k_tb_anon_keys<<<grid(ctx, n_keys), TT, 0, ctx->stream>>>(n_keys, keys, named, niels, key_status);
+        ZK_CUDA(cudaGetLastError());
+    }
+    k_tb_anon_rows<<<grid(ctx, n), TT, 0, ctx->stream>>>(n, sks, rings, positions, amounts, rs, alphas, n_keys, key_status, table, scratch,
+                                                         fields, rsks, dks, status, ctx->d_err);
+    ZK_CUDA(cudaGetLastError());
+    k_tb_anon_lefts<<<grid(ctx, TB_RING_IN * n), TT, 0, ctx->stream>>>(n, keys, rings, positions, amounts, sks, rs, alphas, niels, status,
+                                                                       fields);
+    ZK_CUDA(cudaGetLastError());
+    return ZK_OK;
+}
+
+extern "C" int zk_anonymous_fields_batch_device(zk_ctx *ctx, size_t n_keys, const uint8_t *d_keys, size_t n, const uint8_t *d_sks,
+                                                const uint32_t *d_rings, const uint8_t *d_positions, const uint32_t *d_amounts,
+                                                const uint8_t *d_rs, const uint8_t *d_alphas, const uint8_t *d_g_epoch, uint8_t *d_fields,
+                                                uint8_t *d_rsks, uint8_t *d_dks, uint8_t *d_status) {
+    static const char *fn = "zk_anonymous_fields_batch_device";
+    if (!ctx || (n_keys && !d_keys) || (n && (!d_sks || !d_rings || !d_positions || !d_amounts || !d_rs || !d_alphas || !d_g_epoch ||
+                                              !d_fields || !d_rsks || !d_dks || !d_status))) {
+        zk_set_error("%s: NULL argument", fn);
+        return ZK_ERR_INVALID;
+    }
+    ZK_TRY(check_anon_sizes(fn, n_keys, n));
+    if (!n) return ZK_OK;
+    ZK_TRY(zk_use_device(ctx));
+    return launch_anon(ctx, n_keys, d_keys, n, d_sks, d_rings, d_positions, d_amounts, d_rs, d_alphas, d_g_epoch, d_fields, d_rsks, d_dks,
+                       d_status);
+}
+
+extern "C" int zk_anonymous_fields_batch(zk_ctx *ctx, size_t n_keys, const uint8_t *keys, size_t n, const uint8_t *sks, const uint32_t *rings,
+                                         const uint8_t *positions, const uint32_t *amounts, const uint8_t *rs, const uint8_t *alphas,
+                                         const uint8_t *g_epoch, uint8_t *fields, uint8_t *rsks, uint8_t *dks, uint8_t *status) {
+    static const char *fn = "zk_anonymous_fields_batch";
+    if (!ctx || (n_keys && !keys) || (n && (!sks || !rings || !positions || !amounts || !rs || !alphas || !g_epoch || !fields || !rsks ||
+                                            !dks || !status))) {
+        zk_set_error("%s: NULL argument", fn);
+        return ZK_ERR_INVALID;
+    }
+    ZK_TRY(check_anon_sizes(fn, n_keys, n));
+    if (!n) return ZK_OK;
+    ZK_TRY(check_scalars(fn, "sks", n, sks));
+    ZK_TRY(check_scalars(fn, "rs", n, rs));
+    ZK_TRY(check_scalars(fn, "alphas", n, alphas));
+    ZK_TRY(zk_use_device(ctx));
+    const uint8_t *d_keys, *d_sks, *d_pos, *d_rs, *d_al, *d_g;
+    const uint32_t *d_rings, *d_am;
+    uint8_t *d_fields, *d_rsks, *d_dks, *d_st;
+    Stage io;
+    io.in(keys, d_keys, 32 * n_keys); io.in(sks, d_sks, 32 * n); io.in(rings, d_rings, TB_RING_IN * n); io.in(positions, d_pos, 2 * n);
+    io.in(amounts, d_am, n); io.in(rs, d_rs, 32 * n); io.in(alphas, d_al, 32 * n); io.in(g_epoch, d_g, 32);
+    io.out(fields, d_fields, 32 * TB_N_ANON_FIELDS * n); io.out(rsks, d_rsks, 32 * n); io.out(dks, d_dks, 32 * n); io.out(status, d_st, n);
+    ZK_TRY(io.up(ctx));
+    ZK_TRY(launch_anon(ctx, n_keys, d_keys, n, d_sks, d_rings, d_pos, d_am, d_rs, d_al, d_g, d_fields, d_rsks, d_dks, d_st));
     ZK_TRY(io.down(ctx));
     const int rc = zk_check_err_flag(ctx);   // synchronises the stream
     if (rc == ZK_ERR_DECODE) zk_set_error("%s: g_epoch fails Point::read or is not of prime order", fn);

@@ -11,6 +11,7 @@
 //   rvk, rsk                  pgk + alpha P_G, sk + alpha                                     lib.rs:167-177, redjubjub.rs:58-62
 //   nonce                     dk g_epoch                                                      core/proofs/src/confidential.rs:131
 //   PrivateKey::sign          r = H*(T || M), R = r P_G, S = r + H*(Rbar || M) sk             redjubjub.rs:73-103
+//   the anonymous transfer    neg_encrypt / encrypt / encrypt(0) in gen_proof's ring order     core/proofs/src/anonymous.rs:97-145
 //
 // Every multiple of P_G goes through one fixed-base multiplication: signed 4-bit digits (63 windows of a scalar < 2^252
 // and a carry window), one mixed addition per window from the table d 16^j P_G, d <= 8 (pg_table.inc, global memory,
@@ -354,6 +355,109 @@ ZK_DEV int confidential_fields(const uint32_t *sk_w, const uint32_t *ekr_w, uint
     store_le_words(rsk_out, rsk.l, 8);
     store_le_words(dk_out, dk.l, 8);
     return JJ_OK;
+}
+
+// ---- the anonymous transfer's fields ------------------------------------------------------------------------------------
+// zk_anonymous_fields_batch (tx_build.cu) runs a row in two passes: anonymous_row (one thread per row) computes what the
+// sender's keys give, the sender's slot of both arrays, right_ciphertext, rvk and nonce; anonymous_left (one thread per
+// ring entry) computes r ek for the recipient and each decoy from the call's key table, decoded once per distinct key
+// (anon_key_entry).  Restates MultiCiphertexts::<Anonymous>::encrypt (core/proofs/src/crypto_components.rs:168-216):
+//   sender     neg_encrypt: -amount P_G + r ek_s = (r dk - amount) P_G, because ek_s = dk P_G    core/crypto/src/elgamal.rs:70-85
+//   recipient  encrypt: amount P_G + r ek_t
+//   decoys     encrypt(0): r ek_d
+// and places the entries where gen_proof's two Vec::insert calls put them (core/proofs/src/anonymous.rs:118-145).
+constexpr int TB_RING = 12;                       // ANONIMITY_SIZE
+constexpr int TB_RING_IN = TB_RING - 1;           // ring indices per row: the recipient, then the ten decoys
+constexpr int TB_N_ANON_FIELDS = 2 * TB_RING + 3; // enc_keys[12] | left_ciphertexts[12] | right_ciphertext | rvk | nonce
+constexpr int TB_ANON_BAD_INDEX = 4, TB_ANON_BAD_POSITIONS = 5;
+
+// The ring position of MultiEncKeys entry j (0: the recipient, 1 .. 10: the decoys in order) with the sender at s and the
+// recipient at t (s != t, both < 12).  Inserting the sender at s and the recipient at t into the ten decoys, in either
+// order gen_proof uses, leaves the decoys in their order on the ten other positions.
+ZK_DEV int anon_position(int s, int t, int j) {
+    if (j == 0) return t;
+    const int lo = s < t ? s : t, hi = s < t ? t : s;
+    int p = j - 1;
+    p += p >= lo;
+    p += p >= hi;
+    return p;
+}
+
+// EncryptionKey::read (Point::read + as_prime_order) of one key of the call's table: its JJ status, and its Niels form in
+// out (TB_ENTRY_WORDS words, the layout load_niels reads; the identity's when the read fails)
+ZK_DEV int anon_key_entry(const uint32_t *enc, uint32_t *out) {
+    Ext p;
+    const int st = read_prime_order(enc, p);
+    const Niels q = st == JJ_OK ? niels_of(p.x, p.y, jj_d2()) : niels_identity();
+#pragma unroll
+    for (int i = 0; i < 8; i++) { out[i] = q.ymx.l[i]; out[8 + i] = q.ypx.l[i]; out[16 + i] = q.kt.l[i]; }
+    return st;
+}
+
+// A row's status: TB_ANON_BAD_POSITIONS for s >= 12, t >= 12 or s = t; else TB_ANON_BAD_INDEX for a ring index >= n_keys;
+// else the zk_jubjub_into_xy code of the first key, in MultiEncKeys order, that fails EncryptionKey::read; else 0.
+ZK_DEV int anon_status(int s, int t, const uint32_t *ring, size_t n_keys, const uint8_t *key_status) {
+    if (s >= TB_RING || t >= TB_RING || s == t) return TB_ANON_BAD_POSITIONS;
+#pragma unroll 1
+    for (int j = 0; j < TB_RING_IN; j++)
+        if (ring[j] >= n_keys) return TB_ANON_BAD_INDEX;
+#pragma unroll 1
+    for (int j = 0; j < TB_RING_IN; j++)
+        if (key_status[ring[j]] != JJ_OK) return key_status[ring[j]];
+    return JJ_OK;
+}
+
+// The row pass of one row: status from anon_status, sk / r / alpha < r_J, the sender at s.  A row with status 0 gets
+// enc_keys[s] = ek_s, left_ciphertexts[s], right_ciphertext = r P_G, rvk = rsk P_G, nonce = dk g_epoch (g_table: the
+// g_epoch's window table), rsk and dk; the five points are made affine with one inversion, their X, Y, Z and Z-prefix
+// products parked in scratch (TB_ANON_SCRATCH_SLOTS slots) as in confidential_fields.  A row with another status gets
+// zeros in all TB_N_ANON_FIELDS fields, rsk and dk, and anonymous_left leaves it alone.
+constexpr int TB_ANON_SCRATCH_SLOTS = 20;
+ZK_DEV void anonymous_row(int status, int s, const uint32_t *sk_w, uint32_t amount, const uint32_t *r_w, const uint32_t *alpha_w,
+                          const uint32_t *__restrict__ g_table, uint32_t *scratch, size_t stride, uint8_t *fields, uint8_t *rsk_out,
+                          uint8_t *dk_out) {
+    if (status != JJ_OK) {
+        for (int i = 0; i < 32 * TB_N_ANON_FIELDS; i++) fields[i] = 0;
+        for (int i = 0; i < 32; i++) rsk_out[i] = dk_out[i] = 0;
+        return;
+    }
+    const Fs sk = fs_words(sk_w), r = fs_words(r_w), rsk = sk + fs_words(alpha_w);
+    const Fs dk = decryption_key(sk);
+    Fr acc = Fr::one();
+    auto stash = [&](int k, const Ext &p) {
+        tb_put(scratch, stride, 4 * k, p.x); tb_put(scratch, stride, 4 * k + 1, p.y);
+        tb_put(scratch, stride, 4 * k + 2, p.z); tb_put(scratch, stride, 4 * k + 3, acc);
+        acc = acc * p.z;
+    };
+    stash(0, pg_mul(dk));                                     // enc_keys[s] = ek_s
+    stash(1, pg_mul(fs_mul(r, dk) - fs_u32(amount)));         // left_ciphertexts[s] = -amount P_G + r ek_s
+    stash(2, pg_mul(r));                                      // right_ciphertext = r P_G
+    stash(3, pg_mul(rsk));                                    // rvk = pgk + alpha P_G
+    stash(4, fb_mul<TB_WINDOWS>(g_table, dk.l));              // nonce = dk g_epoch
+    Fr inv = acc.inverse();
+#pragma unroll 1
+    for (int k = 4; k >= 0; k--) {
+        const Fr zi = inv * tb_get(scratch, stride, 4 * k + 3);
+        inv = inv * tb_get(scratch, stride, 4 * k + 2);
+        uint32_t enc[8];
+        jubjub_encode(tb_get(scratch, stride, 4 * k) * zi, tb_get(scratch, stride, 4 * k + 1) * zi, enc);
+        const int slot = k == 0 ? s : k == 1 ? TB_RING + s : 2 * TB_RING + k - 2;
+        store_le_words(fields + 32 * slot, enc, 8);
+    }
+    store_le_words(rsk_out, rsk.l, 8);
+    store_le_words(dk_out, dk.l, 8);
+}
+
+// Ring entry j of a row with status 0, at ring position p (anon_position): q is the entry's key in Niels form and key_enc
+// its 32 table bytes, copied to enc_keys[p]; left_ciphertexts[p] = r key + amount P_G for the recipient (j = 0) and r key
+// + 0 P_G for a decoy (the same 63 products in every lane of a warp, so no branch diverges).
+ZK_DEV void anonymous_left(const Niels &q, const uint8_t *key_enc, int j, int p, uint32_t amount, const uint32_t *r_w, uint8_t *fields) {
+    for (int i = 0; i < 32; i++) fields[32 * p + i] = key_enc[i];
+    uint8_t *out = fields + 32 * (TB_RING + p);
+    const uint32_t aw[8] = {j == 0 ? amount : 0u, 0, 0, 0, 0, 0, 0, 0};
+    uint32_t enc[8];
+    ext_encode(fb_mul<9>(TB_PG_TABLE, aw, vb_mul(q, r_w)), enc);
+    store_le_words(out, enc, 8);
 }
 
 }  // namespace zktb

@@ -631,6 +631,49 @@ def confidential_fields_device(ctx: Context, n: int, d_sks_ptr: int, d_eks_recip
         d_dks_ptr, d_status_ptr))))
 
 
+# zk_anonymous_fields_batch: the 27 points of a row, enc_keys and left_ciphertexts 12 each, in AnonymousTx's argument order
+ANONYMOUS_FIELDS = ("enc_keys", "left_ciphertexts", "right_ciphertext", "rvk", "nonce")
+ANON_BAD_INDEX, ANON_BAD_POSITIONS = 4, 5     # zk_anonymous_fields_batch statuses besides the zk_jubjub_into_xy codes
+
+
+def anonymous_fields(ctx: Context, keys, sks, rings, positions, amounts, rs, alphas, g_epoch_enc):
+    """The ciphertexts, rvk and nonce of n anonymous transfers (MultiCiphertexts::<Anonymous>::encrypt in gen_proof's ring
+    order, and ProofContext): keys the table of 32-byte encryption keys the rings index; sks / rs / alphas scalars < r_J
+    (ints or 32 bytes); rings n rows of 11 indices (recipient, then the ten decoys); positions n pairs (s_index, t_index);
+    amounts uint32; g_epoch_enc the call's 32-byte g_epoch.  Returns (fields, rsks, dks, status): fields[i] is a dict of
+    the ANONYMOUS_FIELDS, enc_keys and left_ciphertexts lists of 12 (AnonymousTx(members, fields[i]["left_ciphertexts"],
+    ...) builds the extrinsic, members being the accounts of enc_keys); rsks / dks 32-byte values; status 0, a
+    zk_jubjub_into_xy code, ANON_BAD_INDEX or ANON_BAD_POSITIONS (non-zero: the row is zero)."""
+    n = len(amounts)
+    ky = _cat(keys, 32)
+    sk, r, al = _scalars(sks, n), _scalars(rs, n), _scalars(alphas, n)
+    rg = np.ascontiguousarray(np.asarray(rings, np.int64).reshape(-1).astype(np.uint32)) if n else np.zeros(1, np.uint32)
+    pos = np.ascontiguousarray(np.asarray(positions, np.int64).reshape(-1).astype(np.uint8)) if n else np.zeros(1, np.uint8)
+    assert (len(rg) == 11 * n and len(pos) == 2 * n) or not n
+    am = np.ascontiguousarray(amounts, np.uint32) if n else np.zeros(1, np.uint32)
+    f = np.zeros(max(864 * n, 1), np.uint8)
+    rsk, dk, st = np.zeros(max(32 * n, 1), np.uint8), np.zeros(max(32 * n, 1), np.uint8), np.zeros(max(n, 1), np.uint8)
+    _ck(_lib.lib().zk_anonymous_fields_batch(ctx._h, len(ky) // 32, _p(_buf(ky)), n, _p(_buf(sk)), _p(rg), _p(pos), _p(am), _p(_buf(r)),
+                                             _p(_buf(al)), _p(_buf(_pt32(g_epoch_enc))), _p(f), _p(rsk), _p(dk), _p(st)))
+    fields = []
+    for i in range(n):
+        pts = _rows(f[864 * i:864 * (i + 1)], 32, 27)
+        fields.append(dict(zip(ANONYMOUS_FIELDS, [pts[:12], pts[12:24], pts[24], pts[25], pts[26]])))
+    return fields, _rows(rsk, 32, n), _rows(dk, 32, n), [int(s) for s in st[:n]]
+
+
+def anonymous_fields_device(ctx: Context, n_keys: int, d_keys_ptr: int, n: int, d_sks_ptr: int, d_rings_ptr: int, d_positions_ptr: int,
+                            d_amounts_ptr: int, d_rs_ptr: int, d_alphas_ptr: int, d_g_epoch_ptr: int, d_fields_ptr: int, d_rsks_ptr: int,
+                            d_dks_ptr: int, d_status_ptr: int):
+    """The same on device pointers (d_keys: n_keys * 32 bytes, 0 when n_keys = 0; d_rings: n * 11 uint32; d_positions:
+    n * 2 bytes; d_amounts: n uint32; d_fields: n * 864 bytes), asynchronous on the context's stream; ctx.sync() raises
+    ZK_ERR_NOT_CANONICAL or ZK_ERR_DECODE (g_epoch)."""
+    v = lambda x: C.c_void_p(x) if x else None
+    _ck(_lib.lib().zk_anonymous_fields_batch_device(ctx._h, n_keys, v(d_keys_ptr), n, *(v(p) for p in (
+        d_sks_ptr, d_rings_ptr, d_positions_ptr, d_amounts_ptr, d_rs_ptr, d_alphas_ptr, d_g_epoch_ptr, d_fields_ptr, d_rsks_ptr, d_dks_ptr,
+        d_status_ptr))))
+
+
 def redjubjub_sign(ctx: Context, sks, msgs, ts) -> list:
     """PrivateKey::sign(msg, rng, FixedGenerators::Diversifier) (core/jubjub/src/redjubjub.rs:73-103) of each message, with
     the 80 bytes ts[i] in place of the RNG's output (draw them with secrets.token_bytes(80)).  sks: scalars < r_J (ints or
