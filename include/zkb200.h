@@ -382,6 +382,50 @@ int zk_redjubjub_sign_batch(zk_ctx *ctx, size_t n, const uint8_t *sks, const uin
  * and the next zk_ctx_sync reports ZK_ERR_NOT_CANONICAL. */
 int zk_redjubjub_sign_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_sks, const uint8_t *d_ts, const uint8_t *d_msgs,
                                    const uint64_t *d_msg_off, uint8_t *d_sigs);
+/* ---- wallet keys: zface's hierarchical key derivation (zface/src/derive/mod.rs, a ZIP-32-style scheme) ----------------
+ * An extended key is written as 73 B: depth u8 | parent tag 4 B | child index u32 LE | chain code 32 B | key 32 B, the key an
+ * sk (32 B Fs, an xsk) or a pgk (a Point::write encoding, an xpgk).  Child indices are raw u32: >= 2^31 is hardened.  All
+ * multiples are of the Diversifier generator P_G.  dks / eks are an account's into_decryption_key(pgk) and dk P_G, the
+ * keys zk_elgamal_decrypt_batch and zk_confidential_fields_batch take; ek is the account's address.
+ * ExtendedSpendingKey::master(seeds[i]) (derive/mod.rs:48-64) for n seeds of any length, laid out as in
+ * zk_keys_from_seed_batch.  xsks: n * 73 B.  xpgks (n * 73 B, From<&ExtendedSpendingKey>: the same header with key =
+ * sk P_G), dks and eks (n * 32 B) are optional: NULL means not computed.  ZK_ERR_INVALID for a required NULL pointer with
+ * n > 0, or for offsets that decrease. */
+int zk_xsk_master_batch(zk_ctx *ctx, size_t n, const uint8_t *seeds, const uint64_t *seed_off, uint8_t *xsks, uint8_t *xpgks,
+                        uint8_t *dks, uint8_t *eks);
+/* the same with device pointers; asynchronous on the context's stream.  The offsets are not checked: they must not decrease. */
+int zk_xsk_master_batch_device(zk_ctx *ctx, size_t n, const uint8_t *d_seeds, const uint64_t *d_seed_off, uint8_t *d_xsks,
+                               uint8_t *d_xpgks, uint8_t *d_dks, uint8_t *d_eks);
+/* ExtendedSpendingKey::derive_child (derive/mod.rs:66-104) for n rows: row i derives child child_idx[i] of the xsk
+ * parents[parent_idx[i]] (parents: a table of n_parents xsks, NULL only when n_parents = 0).  Scanning accounts is one
+ * parent with many indices; a path is one call per level, the previous level's xsks being the next level's parents.
+ * Every parent an in-range row names is read once per call (its sk, pgk and tag); the others are not read.
+ * xsks: n * 73 B; xpgks (n * 73 B), dks and eks (n * 32 B) as in zk_xsk_master_batch, optional.
+ * status[i]: 0 derived; 4 parent_idx >= n_parents; 6 the parent is at depth 255 (its child's depth would not fit in a u8).
+ *   A row with a non-zero status gets all-zero outputs; the other rows are unaffected.
+ * ZK_ERR_NOT_CANONICAL, zk_last_error naming the lowest such parent index, for a named parent whose sk >= r_J
+ * (SpendingKey::read fails); ZK_ERR_INVALID for a required NULL pointer, and for n above 2^26 or n_parents above 2^24. */
+int zk_xsk_derive_batch(zk_ctx *ctx, size_t n_parents, const uint8_t *parents, size_t n, const uint32_t *parent_idx,
+                        const uint32_t *child_idx, uint8_t *xsks, uint8_t *xpgks, uint8_t *dks, uint8_t *eks, uint8_t *status);
+/* the same with device pointers (d_parent_idx and d_child_idx 4-byte aligned); asynchronous on the context's stream.  The
+ * rows that name a parent whose sk >= r_J are left unwritten, status included, and the next zk_ctx_sync reports
+ * ZK_ERR_NOT_CANONICAL.  No output may overlap d_parents: rows read their parents while other rows write, so a path chains
+ * levels through separate buffers, never in place. */
+int zk_xsk_derive_batch_device(zk_ctx *ctx, size_t n_parents, const uint8_t *d_parents, size_t n, const uint32_t *d_parent_idx,
+                               const uint32_t *d_child_idx, uint8_t *d_xsks, uint8_t *d_xpgks, uint8_t *d_dks, uint8_t *d_eks,
+                               uint8_t *d_status);
+/* ExtendedProofGenerationKey::derive_child (derive/mod.rs:164-197), the watch-only derivation: parents is a table of
+ * n_parents xpgks, and the rows work as in zk_xsk_derive_batch.  xpgks: n * 73 B; dks and eks (n * 32 B) optional.
+ * status[i]: 0 derived; 4 parent_idx >= n_parents; else 1 / 2 / 3, the zk_jubjub_into_xy code of a parent whose pgk fails
+ *   ProofGenerationKey::read (Point::read + as_prime_order); else 5 for a hardened index (the reference returns an error);
+ *   else 6 for a parent at depth 255.  A row with a non-zero status gets all-zero outputs; the other rows are unaffected.
+ * ZK_ERR_INVALID for a required NULL pointer, and for n above 2^26 or n_parents above 2^24. */
+int zk_xpgk_derive_batch(zk_ctx *ctx, size_t n_parents, const uint8_t *parents, size_t n, const uint32_t *parent_idx,
+                         const uint32_t *child_idx, uint8_t *xpgks, uint8_t *dks, uint8_t *eks, uint8_t *status);
+/* the same with device pointers (d_parent_idx and d_child_idx 4-byte aligned); asynchronous on the context's stream.  As in
+ * zk_xsk_derive_batch_device, no output may overlap d_parents. */
+int zk_xpgk_derive_batch_device(zk_ctx *ctx, size_t n_parents, const uint8_t *d_parents, size_t n, const uint32_t *d_parent_idx,
+                                const uint32_t *d_child_idx, uint8_t *d_xpgks, uint8_t *d_dks, uint8_t *d_eks, uint8_t *d_status);
 /* ---- confidential-transfer balance updates of one block (what modules/encrypted-balances runs around each proof) ------
  * rollover + sub_enc_balance + add_pending_transfer (modules/encrypted-balances/src/lib.rs:25-96, 133-222) for n_tx
  * transactions, in order, over a table of n_accounts accounts.

@@ -87,6 +87,12 @@ SIGNATURES = {
     "zk_anonymous_fields_batch_device": (i32, [vp, sz, vp, sz] + [vp] * 11),
     "zk_redjubjub_sign_batch": (i32, [vp, sz, vp, vp, vp, vp, vp]),
     "zk_redjubjub_sign_batch_device": (i32, [vp, sz, vp, vp, vp, vp, vp]),
+    "zk_xsk_master_batch": (i32, [vp, sz] + [vp] * 6),
+    "zk_xsk_master_batch_device": (i32, [vp, sz] + [vp] * 6),
+    "zk_xsk_derive_batch": (i32, [vp, sz, vp, sz] + [vp] * 7),
+    "zk_xsk_derive_batch_device": (i32, [vp, sz, vp, sz] + [vp] * 7),
+    "zk_xpgk_derive_batch": (i32, [vp, sz, vp, sz] + [vp] * 6),
+    "zk_xpgk_derive_batch_device": (i32, [vp, sz, vp, sz] + [vp] * 6),
     "zk_balances_confidential_block": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_confidential_block_device": (i32, [vp, sz, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "zk_balances_anonymous_block": (i32, [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -57,7 +57,7 @@ extern "C" void zk_ctx_destroy(zk_ctx *c) {
                       &c->stage_c, &c->ntt_tmp, &c->g_a, &c->g_b, &c->g_c, &c->g_h, &c->g_scal, &c->g_misc,
                       &c->aff_pts0, &c->aff_pts1, &c->aff_scratch, &c->aff_off0, &c->aff_off1, &c->aff_sizes0, &c->aff_sizes1, &c->aff_tot, &c->red_rows, &c->g_scal2, &c->g_scal3, &c->sorted2, &c->coarse_off, &c->coarse_sizes, &c->task_order, &c->len_hist, &c->heavy_list, &c->red_tmp,
                       &c->v_pts, &c->v_stat, &c->v_coef, &c->v_f, &c->v_part, &c->v_jj,
-                      &c->eg_table, &c->eg_index, &c->jm, &c->bal, &c->imp, &c->io, &c->imp_as, &c->tb};
+                      &c->eg_table, &c->eg_index, &c->jm, &c->bal, &c->imp, &c->io, &c->imp_as, &c->tb, &c->hd};
     for (DevBuf *b : bufs) b->release();
     for (NttSlot &sl : c->ntt_slots) { sl.w.release(); sl.g.release(); sl.gi.release(); sl.consts.release(); }
     if (c->tail) { cudaStreamSynchronize(c->tail); cudaStreamDestroy(c->tail); cudaEventDestroy(c->ev_front); cudaEventDestroy(c->ev_tail); }

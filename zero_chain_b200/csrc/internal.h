@@ -93,6 +93,7 @@ struct zk_ctx {
                                    // synchronises before it returns, so one buffer serves them all
     DevBuf imp_as;                 // zk_import_asset_calls (import.cu): the hash table, references and grown slot table
     DevBuf tb;                     // zk_confidential_fields_batch (tx_build.cu): the g_epoch window table and the rows' points
+    DevBuf hd;                     // zk_xsk_derive_batch / zk_xpgk_derive_batch (hd_keys.cu): each named parent's pgk and tag
     DevBuf jm;                     // zk_jubjub_msm / zk_redjubjub_batch_verify (jubjub_msm.cu): bases, scalars, sort and buckets
     // live kernel timing (zk_ctx_profile): CUDA events around the dominant kernel on ctx->stream
     bool prof_on = false;

@@ -694,6 +694,107 @@ def redjubjub_sign_device(ctx: Context, n: int, d_sks_ptr: int, d_ts_ptr: int, d
                                                   C.c_void_p(d_msg_off_ptr), C.c_void_p(d_sigs_ptr)))
 
 
+# ---- wallet keys: zface's hierarchical key derivation (zface/src/derive/mod.rs) ----------------------------------------
+# An extended key is 73 opaque bytes (ExtendedSpendingKey / ExtendedProofGenerationKey::write); child indices are raw u32,
+# HD_HARDENED and above hardened.  Row statuses of the derive calls besides the zk_jubjub_into_xy codes:
+XK_BYTES = 73
+HD_HARDENED = 1 << 31
+HD_BAD_INDEX, HD_HARDENED_INDEX, HD_DEPTH = 4, 5, 6
+
+
+def _idx32(v, n: int, what: str):
+    """n raw u32 indices; a value outside 0 .. 2^32 - 1 is refused, not wrapped (-1 would become a hardened index)"""
+    if not n:
+        return np.zeros(1, np.uint32)
+    a = [int(x) for x in np.asarray(v, dtype=object).reshape(-1)]
+    if len(a) != n:
+        raise ValueError("%s: %d values for %d rows" % (what, len(a), n))
+    bad = next((i for i, x in enumerate(a) if not 0 <= x < 1 << 32), None)
+    if bad is not None:
+        raise ValueError("%s[%d] = %d is not a u32" % (what, bad, a[bad]))
+    return np.ascontiguousarray(np.array(a, np.uint64).astype(np.uint32))
+
+
+def _opt(want: bool, size: int, n: int):
+    return np.zeros(max(size * n, 1), np.uint8) if want else None
+
+
+def _opt_rows(out, size: int, n: int):
+    return _rows(out, size, n) if out is not None else None
+
+
+def _dptr(p: int):
+    return C.c_void_p(p) if p else None
+
+
+def xsk_master(ctx: Context, seeds, xpgk: bool = True, dk: bool = True, ek: bool = True):
+    """ExtendedSpendingKey::master(seed) of each seed (byte strings of any length, e.g. a bip39 seed) — what zface's
+    `wallet init` / `recover` build.  Returns (xsks, xpgks, dks, eks): xsks 73-byte extended spending keys; xpgks their
+    ExtendedProofGenerationKeys (73 bytes), dks / eks the master account's decryption and encryption keys (32 bytes), each
+    list None when not asked for."""
+    n = len(seeds)
+    xsk, xp, d, e = np.zeros(max(XK_BYTES * n, 1), np.uint8), _opt(xpgk, XK_BYTES, n), _opt(dk, 32, n), _opt(ek, 32, n)
+    _ck(_lib.lib().zk_xsk_master_batch(ctx._h, n, _p(_buf(b"".join(bytes(s) for s in seeds))), _p(message_offsets(seeds)), _p(xsk),
+                                       *(_p(a) if a is not None else None for a in (xp, d, e))))
+    return _rows(xsk, XK_BYTES, n), _opt_rows(xp, XK_BYTES, n), _opt_rows(d, 32, n), _opt_rows(e, 32, n)
+
+
+def xsk_master_device(ctx: Context, n: int, d_seeds_ptr: int, d_seed_off_ptr: int, d_xsks_ptr: int, d_xpgks_ptr: int = 0,
+                      d_dks_ptr: int = 0, d_eks_ptr: int = 0):
+    """The same on device pointers (d_seed_off: n + 1 uint64 offsets; 0 for an output not wanted), asynchronous on the
+    context's stream."""
+    _ck(_lib.lib().zk_xsk_master_batch_device(ctx._h, n, *(_dptr(p) for p in (d_seeds_ptr, d_seed_off_ptr, d_xsks_ptr, d_xpgks_ptr, d_dks_ptr,
+                                                                                d_eks_ptr))))
+
+
+def xsk_derive(ctx: Context, parents, parent_idx, child_idx, xpgk: bool = True, dk: bool = True, ek: bool = True):
+    """ExtendedSpendingKey::derive_child: row i derives child child_idx[i] (a raw u32, >= HD_HARDENED hardened) of
+    parents[parent_idx[i]], parents being 73-byte xsks (a list, or their concatenation).  Account k of a wallet is
+    xsk_derive(ctx, [master], [0], [k]).  Returns (xsks, xpgks, dks, eks, status): as xsk_master, and status 0,
+    HD_BAD_INDEX or HD_DEPTH per row (non-zero: the row is zero).  Raises ZK_ERR_NOT_CANONICAL naming the parent when a
+    named parent's sk >= r_J."""
+    pb = _cat(parents, XK_BYTES)
+    n = len(parent_idx)
+    pi, ci = _idx32(parent_idx, n, "parent_idx"), _idx32(child_idx, n, "child_idx")
+    xsk, st = np.zeros(max(XK_BYTES * n, 1), np.uint8), np.zeros(max(n, 1), np.uint8)
+    xp, d, e = _opt(xpgk, XK_BYTES, n), _opt(dk, 32, n), _opt(ek, 32, n)
+    _ck(_lib.lib().zk_xsk_derive_batch(ctx._h, len(pb) // XK_BYTES, _p(_buf(pb)), n, _p(pi), _p(ci), _p(xsk),
+                                       *(_p(a) if a is not None else None for a in (xp, d, e)), _p(st)))
+    return _rows(xsk, XK_BYTES, n), _opt_rows(xp, XK_BYTES, n), _opt_rows(d, 32, n), _opt_rows(e, 32, n), [int(s) for s in st[:n]]
+
+
+def xsk_derive_device(ctx: Context, n_parents: int, d_parents_ptr: int, n: int, d_parent_idx_ptr: int, d_child_idx_ptr: int,
+                      d_xsks_ptr: int, d_xpgks_ptr: int, d_dks_ptr: int, d_eks_ptr: int, d_status_ptr: int):
+    """The same on device pointers (d_parents: n_parents * 73 bytes; d_parent_idx / d_child_idx: n uint32; 0 for an output
+    not wanted), asynchronous on the context's stream; ctx.sync() raises ZK_ERR_NOT_CANONICAL for a named parent whose
+    sk >= r_J, whose rows are left unwritten.  A path chains calls, each level's d_xsks the next level's d_parents; no
+    output may overlap d_parents."""
+    _ck(_lib.lib().zk_xsk_derive_batch_device(ctx._h, n_parents, _dptr(d_parents_ptr), n, *(_dptr(p) for p in (
+        d_parent_idx_ptr, d_child_idx_ptr, d_xsks_ptr, d_xpgks_ptr, d_dks_ptr, d_eks_ptr, d_status_ptr))))
+
+
+def xpgk_derive(ctx: Context, parents, parent_idx, child_idx, dk: bool = True, ek: bool = True):
+    """ExtendedProofGenerationKey::derive_child, the watch-only derivation: as xsk_derive over 73-byte xpgk parents, with
+    no spending key.  Returns (xpgks, dks, eks, status): status 0; HD_BAD_INDEX; the zk_jubjub_into_xy code (1 / 2 / 3)
+    of a parent whose pgk fails ProofGenerationKey::read; HD_HARDENED_INDEX; or HD_DEPTH (non-zero: the row is zero).
+    The dks decrypt the derived accounts' balances with elgamal_decrypt."""
+    pb = _cat(parents, XK_BYTES)
+    n = len(parent_idx)
+    pi, ci = _idx32(parent_idx, n, "parent_idx"), _idx32(child_idx, n, "child_idx")
+    xp, st = np.zeros(max(XK_BYTES * n, 1), np.uint8), np.zeros(max(n, 1), np.uint8)
+    d, e = _opt(dk, 32, n), _opt(ek, 32, n)
+    _ck(_lib.lib().zk_xpgk_derive_batch(ctx._h, len(pb) // XK_BYTES, _p(_buf(pb)), n, _p(pi), _p(ci), _p(xp),
+                                        *(_p(a) if a is not None else None for a in (d, e)), _p(st)))
+    return _rows(xp, XK_BYTES, n), _opt_rows(d, 32, n), _opt_rows(e, 32, n), [int(s) for s in st[:n]]
+
+
+def xpgk_derive_device(ctx: Context, n_parents: int, d_parents_ptr: int, n: int, d_parent_idx_ptr: int, d_child_idx_ptr: int,
+                       d_xpgks_ptr: int, d_dks_ptr: int, d_eks_ptr: int, d_status_ptr: int):
+    """The same on device pointers, as xsk_derive_device; asynchronous on the context's stream."""
+    _ck(_lib.lib().zk_xpgk_derive_batch_device(ctx._h, n_parents, _dptr(d_parents_ptr), n, *(_dptr(p) for p in (
+        d_parent_idx_ptr, d_child_idx_ptr, d_xpgks_ptr, d_dks_ptr, d_eks_ptr, d_status_ptr))))
+
+
 # ---- confidential-transfer balance updates of one block (modules/encrypted-balances/src/lib.rs:25-96, 133-222) ----------
 # account flags and zk_balances_confidential_block statuses
 ACCOUNT_BALANCE, ACCOUNT_PENDING, ACCOUNT_DUE = 1, 2, 4
